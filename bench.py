@@ -27,8 +27,6 @@ sys.path.insert(0, ROOT)
 from hivedscheduler_b200 import _cabi, trace  # noqa: E402
 
 METRIC = "scheduling decisions/sec on 64k-GPU cell tree, 100k pending gangs"
-# dram__bytes_read.sum + dram__bytes_write.sum of hived_events_kernel over the full C3 trace (one ncu --set full capture)
-NCU_DRAM_BYTES_PER_LAUNCH_C3 = 88_998_912 + 93_801_728  # profiles/r2_final.md section 2 (the final kernel)
 WORKLOAD = "C3: 8192 nodes x 8 GPU (65536 GPUs), 5-level tree, 8 VCs, 100000 mixed gangs (1/4/8/64-GPU), admission window 0.9"
 
 
@@ -39,11 +37,11 @@ def measured_peak_gbs():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet: 3.35 TB/s of HBM3)"
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks + throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks, throttle reasons and the power limit during the timed region."""
 
     def __init__(self, device: int):
         super().__init__(daemon=True)
@@ -53,7 +51,7 @@ class ClockSampler(threading.Thread):
 
     def run(self):
         q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
-             "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
+             "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit")
         while not self.stop_flag.is_set():
             try:
                 out = subprocess.check_output(["nvidia-smi", "-i", str(self.device), "--query-gpu=" + q,
@@ -65,12 +63,14 @@ class ClockSampler(threading.Thread):
 
     def summary(self):
         if not self.samples:
-            return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
+            return {"sm_mhz": None, "sm_max_mhz": None, "power_limit_w": None, "reasons": ["nvidia-smi unavailable"]}
         sm = sorted(int(s[0]) for s in self.samples if s[0].isdigit())
         mx = max(int(s[1]) for s in self.samples if s[1].isdigit())
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         reasons = [n for i, n in enumerate(names) if any(s[2 + i].lower().startswith("active") for s in self.samples)]
-        return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": mx, "reasons": reasons, "samples": len(self.samples)}
+        pl = self.samples[-1][6] if len(self.samples[-1]) > 6 else None
+        return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": mx, "power_limit_w": pl, "reasons": reasons,
+                "samples": len(self.samples)}
 
 
 def bind_bench_hooks(lib):
@@ -89,6 +89,27 @@ def bind_bench_hooks(lib):
         fn = getattr(lib, name)
         fn.restype = res
         fn.argtypes = args
+
+
+DUMP_BYTES = 64_000_000
+
+
+def dump_outputs(out_dir, res, pool):
+    """What the timed path returned in its last step, as float64 .npy files of at most DUMP_BYTES in all: the words of
+    the result pool and the hived_result_t records that point into it (one row per event, one column per int32 word).
+    The pool gets at most half of the budget and the records whatever the pool leaves; an output larger than its share is
+    cut to a fixed sample (numpy seed 0) of words / rows, and the indices of what was kept are written beside it
+    (pool_index.npy, results_rows.npy)."""
+    os.makedirs(out_dir, exist_ok=True)
+    rows = res.view(np.int32).reshape(len(res), res.dtype.itemsize // 4)
+    budget = DUMP_BYTES - 4 * 128  # the four .npy headers
+    for name, arr, index_name, share in (("pool", pool, "pool_index", budget // 2), ("results", rows, "results_rows", None)):
+        per = 8 * (arr.shape[1] if arr.ndim > 1 else 1) + 8  # one row or word plus its index
+        keep = min(len(arr), (budget if share is None else share) // per)
+        idx = np.arange(len(arr)) if keep == len(arr) else np.sort(np.random.default_rng(0).choice(len(arr), keep, replace=False))
+        np.save(os.path.join(out_dir, name + ".npy"), arr[idx].astype(np.float64))
+        np.save(os.path.join(out_dir, index_name + ".npy"), idx.astype(np.float64))
+        budget -= keep * per
 
 
 def dist_env():
@@ -165,7 +186,7 @@ def other_configs(lib):
     bc = trace.BatchContext(lib, t["config"], t["n_groups"], t["n_pods"], t["max_group_leaves"], t["max_group_pods"])
     bc.set_all_nodes_healthy()
     # C2 is 10 000 events (about 40 ms): one cold pass is at the mercy of one-time costs of a fresh context (first
-    # multi-CTA launch of it, page faults of the result buffers: 34 k - 250 k decisions/s from box to box), so the trace
+    # multi-CTA launch of it, page faults of the result buffers), so the trace
     # runs three times from the same saved state and the line carries the best pass AND the first one
     lib.hived_bench_save_state(bc.ctx)
     times, h2 = [], None
@@ -481,7 +502,11 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--replicas", action="store_true", help="N > 1: independent replicas (weak scaling) instead of the VC partition")
     ap.add_argument("--no-other-configs", action="store_true", help="skip the C2 / C4 / C5 sub-lines (about 45 s)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the results and result pool of the last timed step of the "
+                                                          "resident leg (the headline value) to DIR as .npy files")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl == "reference" or int(os.environ.get("WORLD_SIZE", "1")) > 1):
+        raise SystemExit("--dump-outputs: only for the single-GPU run of --impl ours")
     if args.impl == "reference":
         return run_reference_arm(args)
 
@@ -558,7 +583,10 @@ def main():
     n_ctas = lib.hived_bench_num_ctas(ctx)
     # parity witness: the hash of the last step's results
     used = C.c_int64()
-    lib.hived_bench_fetch_results(ctx, res_ptr, pool_ptr, pool_words, C.byref(used))
+    assert lib.hived_bench_fetch_results(ctx, res_ptr, pool_ptr, pool_words, C.byref(used)) == 0
+    if args.dump_outputs:  # copied now: the later legs reuse the buffers; written after the last timed leg
+        last_res = np.frombuffer(res_pinned.numpy(), dtype=trace.RESULT_DT).copy()
+        last_pool = pool_pinned.numpy()[:int(used.value)].copy()
     stats = bc.stats()
     cyc = (C.c_int64 * 15)()
     lib.hived_bench_phase_cycles(ctx, cyc)
@@ -598,6 +626,8 @@ def main():
     per_call_s = (time.perf_counter() - t0) / max(1, n_calls - 64)
     per_call_kernel_us = 1e3 * (lib.hived_bench_total_kernel_ms(ctx) - k0) / max(1, n_calls - 64)
     lib.hived_bench_set_result_hash(ctx, 1)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, last_res, last_pool)
 
     times = torch.tensor([kernel_total_s, e2e_s, wall], dtype=torch.float64, device="cuda")
     if world > 1:
@@ -628,11 +658,10 @@ def main():
                              "mapped host memory, no launch / memcpy / stream sync per call); HIVED_NO_RESIDENT=1 = one launch "
                              "per call.  From C: profiles/micro/percall_latency.c"},
         "gpu_launches": int(launches),
+        "gpu": torch.cuda.get_device_name(local),
         "clocks": sampler.summary(),
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                     "traffic": NCU_DRAM_BYTES_PER_LAUNCH_C3 if args.gangs == 100000 else None,
-                     "traffic_source": "ncu --set full, dram__bytes_read.sum + dram__bytes_write.sum of one full-size launch "
-                                       "(profiles/r2_final.md section 2); bytes per launch",
+                     "traffic": None,
                      "algorithmic_bytes_per_launch": int(alg_bytes), "kernel": "hived_events_kernel",
                      "peak_source": peak_src,
                      "note": "latency-bound sequential contract: the state (~9 MB of cells) is L2/L1 resident, DRAM traffic is "

@@ -1,4 +1,4 @@
-"""hivedscheduler_b200 — B200-native implementation of HiveD's scheduling hot path
+"""hivedscheduler_b200 — CUDA-native (H100, sm_90a) implementation of HiveD's scheduling hot path
 (microsoft/hivedscheduler pkg/algorithm) behind the reference's own plugin boundary.
 
 Only what the path needs lives here: ``csrc/`` (CUDA kernels + the C ABI of include/hived.h),

@@ -1,4 +1,4 @@
-// The scheduling program of the B200-native HiveD hot path (device code; see hived_prims.h for
+// The scheduling program of the CUDA-native HiveD hot path (device code; see hived_prims.h for
 // the execution model).  It implements, over the flat HBM-resident arrays of hived_dev.h, the
 // behaviour of the reference's pkg/algorithm (HivedAlgorithm.Schedule -> intra-VC topology-aware
 // search -> buddy-cell virtual->physical mapping -> commit) — each function cites the reference
@@ -87,7 +87,7 @@ __shared__ Sm g_hived_sm;  // one per CTA (both kernels of hived_cuda.cu use it)
 // The device's view of the scheduler state (array pointers and sizes, hived_dev.h) lives in the CONSTANT bank: `d.p_prio[i]`
 // is one load whose base address is an instruction operand (c[3][offset]).  Through a `const Dev&` member the
 // compiler fetched the pointer with a generic load (LD.E.64) before nearly every data load — a dependent L1 round trip
-// on the leader warp's critical path and a third of its memory instructions (profiles/r2_sass_summary.md).  One
+// on the leader warp's critical path and a third of its memory instructions.  One
 // context's Dev is loaded per device at a time; launchProgram / the per-call path reload it when the owner changes
 // (hived_cuda.cu: ensureDevLoaded).
 __constant__ Dev g_hived_dev;
@@ -347,7 +347,7 @@ struct Core {
   // Work counters (ST_VIEW_NODES .. ST_PRIO_MASK): accumulated per CTA in 32-bit slots and added to d.stats when the
   // batch ends (a batch is far below 2^31 of anything).  The SM-cycle counters (ST_CYC_* and the scratch ST_DBG*)
   // exist only in profiling builds (-DHIVED_PROFILE): in the product neither the clock reads nor the updates are
-  // compiled in — they were 6 % of the leader warp's time.
+  // compiled in (they sit on the leader warp's critical path).
   static constexpr int N_WORK = ST_PRIO_MASK;  // counters [0, N_WORK) are the work counters
   int work[N_WORK];
   int pathCnt[PC_COUNT];  // which path the events took (ST_PATH0 + PC_*)

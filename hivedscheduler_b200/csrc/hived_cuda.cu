@@ -1,4 +1,4 @@
-// libhived_cuda.so — the product: CUDA backend (sm_100a) of include/hived.h.
+// libhived_cuda.so — the product: CUDA backend (sm_90a) of include/hived.h.
 //
 // One kernel, `hived_events_kernel`, runs the scheduling program of hived_core.h over an ordered
 // batch of events with ALL scheduler state resident in HBM (hived_dev.h).  It is launched with one
@@ -101,7 +101,7 @@ void bk_flush_l2() {  // one buffer per device (the current one)
   static void* bufs[64] = {nullptr};
   int dv = 0;
   if (cudaGetDevice(&dv) != cudaSuccess || dv < 0 || dv >= 64) return;
-  const size_t bytes = 256u << 20;  // > 126 MB of L2
+  const size_t bytes = 256u << 20;  // several times the 50 MB L2 of an H100
   if (!bufs[dv] && cudaMalloc(&bufs[dv], bytes) != cudaSuccess) { bufs[dv] = nullptr; return; }
   static int v = 0;
   cudaMemset(bufs[dv], ++v & 0xff, bytes);
@@ -277,7 +277,7 @@ int launchProgram(Engine& e, int n, bool withInit) {
 // ---- per-call path ------------------------------------------------------------------------------------------
 // hived_schedule / hived_add_allocated_pod / hived_delete_* and tiny batches: one pinned staging buffer laid out as
 // [events | scalars | suggested bitmaps | aux | results | pool window]; H2D, kernel and D2H are queued on the stream
-// and the host waits once.  (The general path issues ~6 blocking copies: ~100 us per call on B200.)
+// and the host waits once.  (The general path issues ~6 blocking copies per call.)
 struct SmallStage {  // never freed: a few KB of pinned memory per calling thread, and no CUDA call at thread exit
   char* host = nullptr;
   size_t bytes = 0;
@@ -334,7 +334,8 @@ static int serveCall(Engine& e, CudaTimers* t, const hived_event_t* events, int 
   auto launch = [&]() {
     s[SERVE_DONE_OFF + 4] = 0;
     __sync_synchronize();
-    // ~1.5 us per poll over PCIe: leave after about 2 ms without a request
+    // 1500 polls over PCIe: the kernel leaves after 1.5-2 ms without a request on an H100
+    // (profiles/micro/resident_idle_timeout.py)
     hived_serve_kernel<<<1, NT, 0, t->serveStream>>>(t->slotDev, seq - 1, 1500, t->stageRes, t->dSugg, t->dAux, e.nPinnedOrder,
                                                       e.nBad, t->servePool);
     t->alive = true;
@@ -564,4 +565,4 @@ int bk_canonicalise(Engine& e, int n, long long* total) {
 
 }  // namespace hived
 
-extern "C" const char* hived_backend(void) { return "cuda-sm100a"; }
+extern "C" const char* hived_backend(void) { return "cuda-sm90a"; }

@@ -1,4 +1,4 @@
-// Device-resident state of the B200-native HiveD scheduling path: one POD struct of raw pointers
+// Device-resident state of the CUDA-native HiveD scheduling path: one POD struct of raw pointers
 // into HBM (flat int32 SoA, see DESIGN.md "Data layout").  Static arrays come from FlatTopo
 // (hived_topo.hpp); mutable arrays are the scheduler state that the reference keeps in its
 // pointer forest (pkg/algorithm/cell.go:58-142,315-324; hived_algorithm.go:40-105).

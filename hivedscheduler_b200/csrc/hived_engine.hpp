@@ -1,7 +1,7 @@
 // Host side of the library behind include/hived.h: owns the flattened topology, the device memory
 // and the staging buffers; every ABI call becomes an ordered batch of events executed by the device
 // program (hived_core.h).  Included by exactly one translation unit per build:
-//   hived_cuda.cu        -> libhived_cuda.so   (the product: CUDA backend, sm_100a, no host path)
+//   hived_cuda.cu        -> libhived_cuda.so   (the product: CUDA backend, sm_90a, no host path)
 //   tests/emu/hived_emu.cpp -> test-only 1-thread emulation of the same device program (HIVED_EMU)
 // The backend supplies bk_* (memory) and launchProgram().
 #pragma once
@@ -554,7 +554,7 @@ struct Engine {
   // *stopEvent = the first such event among this rank's events below the horizon (the CTA is parked before it), or
   // 0x7fffffff when every owned event below the horizon has run.  The horizon keeps the VCs moving together: without
   // one, a CTA runs on to its own next such event while the others stay parked at theirs, and the whole batch
-  // degenerates to one VC at a time (measured: 8x slower than one GPU).
+  // degenerates to one VC at a time.
   int mgRun(int32_t horizon, int32_t* stopEvent) {
     bk_use_device(deviceOrdinal);
     mgLimit.assign(launchCta, 0);

@@ -1,7 +1,7 @@
 // Execution primitives of the device program.
 //
 // The scheduling program (hived_core.h) is written once against these primitives:
-//   * CUDA build (the product, sm_100a): one CTA; warp 0 is the "leader warp" that executes the
+//   * CUDA build (the product, sm_90a): one CTA; warp 0 is the "leader warp" that executes the
 //     sequential control flow warp-uniformly (all 32 lanes run the same scalar code; stores are
 //     done by lane 0 and ordered with __syncwarp), the other warps sleep in the hardware barrier
 //     until the leader posts a data-parallel operation (cluster-view pass) in shared memory.

@@ -1,5 +1,5 @@
 /*
- * hived.h — C ABI of the B200-native HiveD scheduling hot path (libhived_cuda.so).
+ * hived.h — C ABI of the CUDA-native HiveD scheduling hot path (libhived_cuda.so).
  *
  * The reference (microsoft/hivedscheduler, Go) has no FFI.  This header is the contract a cgo shim
  * binds so that a Go type implementing internal.SchedulerAlgorithm
@@ -255,7 +255,7 @@ int hived_create(const char* spec_text, const hived_options_t* opt, hived_ctx** 
 void hived_destroy(hived_ctx* ctx);
 const char* hived_last_error(hived_ctx* ctx);       /* valid until the next call on ctx */
 const char* hived_create_error(void);               /* text of the last failed hived_create */
-const char* hived_backend(void);                    /* "cuda-sm100a" | "cpu-oracle" */
+const char* hived_backend(void);                    /* "cuda-sm90a"  | "cpu-oracle" */
 
 /* ---- interning tables */
 int32_t hived_num_nodes(hived_ctx*);       const char* hived_node_name(hived_ctx*, int32_t id);

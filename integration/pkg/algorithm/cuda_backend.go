@@ -3,7 +3,7 @@
 // cuda_backend.go — drop-in file for microsoft/hivedscheduler, pkg/algorithm.
 //
 // CudaHivedAlgorithm implements internal.SchedulerAlgorithm (pkg/internal/types.go:76-100) over the C ABI of
-// include/hived.h (libhived_cuda.so, the B200-native scheduling path).  It keeps in Go exactly what the reference
+// include/hived.h (libhived_cuda.so, the CUDA-native scheduling path).  It keeps in Go exactly what the reference
 // keeps in Go around HivedAlgorithm: the pod-annotation YAML (internal.ExtractPodSchedulingSpec /
 // ExtractPodBindInfo, pkg/internal/utils.go:199-289), the string <-> id interning, the materialisation of
 // api.PodBindInfo / PodWaitInfo / PodPreemptInfo and of the inspect objects.  Everything below the interface —

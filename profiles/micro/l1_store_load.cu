@@ -1,5 +1,5 @@
 // Microbenchmark: does a global store leave the line in L1 for a later load by the same SM?
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o l1_store_load l1_store_load.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o l1_store_load l1_store_load.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 __global__ void k(int* buf, long long* out) {

@@ -35,7 +35,7 @@ GROUPS = [
     ("fences", ("MEMBAR", "FENCE", "ERRBAR", "CCTL")),
     ("branches", ("BRA", "BSSY", "BSYNC", "WARPSYNC", "EXIT")),
 ]
-print("# SASS opcode summary of `%s` (sm_100a)\n" % lib.split("/")[-1])
+print("# SASS opcode summary of `%s` (sm_90a)\n" % lib.split("/")[-1])
 print("Produced by `profiles/scripts/sass_summary.py` from `cuobjdump -sass`; counts are static instructions.\n")
 for f, c in ops.items():
     total = sum(c.values())

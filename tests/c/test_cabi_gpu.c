@@ -52,7 +52,7 @@ int main(int argc, char** argv) {
   hived_ctx* ctx = NULL;
   int rc = hived_create(spec, &opt, &ctx);
   CHECK(rc == 0, "hived_create: %d %s", rc, hived_create_error());
-  if (!getenv("HIVED_TEST_ANY_BACKEND")) CHECK(strcmp(hived_backend(), "cuda-sm100a") == 0, "not the CUDA library: %s", hived_backend());
+  if (!getenv("HIVED_TEST_ANY_BACKEND")) CHECK(strcmp(hived_backend(), "cuda-sm90a") == 0, "not the CUDA library: %s", hived_backend());
   const int vc = find_id(ctx, hived_num_vcs, hived_vc_name, "default");
   const int k80 = find_id(ctx, hived_num_leaf_types, hived_leaf_type_name, "K80");
   const int node23 = find_id(ctx, hived_num_nodes, hived_node_name, "10.151.41.23");

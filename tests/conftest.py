@@ -12,7 +12,7 @@ ORACLE_LIB = os.path.join(ROOT, "oracle", "libhived_oracle.so")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100, sm_90a)")
 
 
 def _build_oracle():

@@ -2,7 +2,7 @@
 // package.  Compiles the product's device program (csrc/hived_core.h) for the host as a
 // 1-thread / 1-lane CTA (HIVED_EMU) behind the same C ABI, so that the kernel LOGIC can be
 // parity-tested against the oracle in a container that has no GPU.  GPU tests (-m gpu) exercise
-// the real sm_100a build; this file exists because GPU round trips are scarce during development.
+// the real sm_90a build; this file exists because GPU round trips are scarce during development.
 #define HIVED_EMU 1
 #include <cstdlib>
 #include <cstring>

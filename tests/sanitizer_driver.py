@@ -1,4 +1,4 @@
-"""Driver for the compute-sanitizer runs (profiles/sanitizer_*.log): a short calm C3-shaped trace with `vcs` virtual
+"""Driver for the compute-sanitizer runs: a short calm C3-shaped trace with `vcs` virtual
 clusters (= CTAs of the VC-parallel launch) and a short C5-shaped churn trace (bad nodes: one CTA), replayed through
 the C ABI on whatever library HIVED_CUDA_LIB / the default build provides; prints the result hashes.
 

@@ -24,7 +24,7 @@ def test_header_symbols_are_bound_and_exported():
     for sym in declared_symbols():
         assert sym in bound, "include/hived.h declares %s but _cabi does not bind it" % sym
         assert getattr(lib, sym) is not None
-    assert lib.hived_backend() == b"cuda-sm100a"
+    assert lib.hived_backend() == b"cuda-sm90a"
     # the other headers of include/: measurement hooks, multi-GPU partition, request ingest
     from hivedscheduler_b200 import dist, frontend, ingest
     dist.bind_multigpu(lib)

@@ -1,5 +1,5 @@
 """Logic parity of the DEVICE PROGRAM (csrc/hived_core.h) against the oracle, executed on the host by
-the test-only 1-thread emulation (tests/emu).  The real sm_100a build is covered by test_gpu_parity.py;
+the test-only 1-thread emulation (tests/emu).  The real sm_90a build is covered by test_gpu_parity.py;
 these tests let kernel-logic regressions show up in the CPU-only CI tier."""
 import numpy as np
 import pytest
