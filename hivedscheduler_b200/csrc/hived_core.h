@@ -443,31 +443,41 @@ struct Core {
     ST(d.p_bfpos[cell], -1);
     ST(d.bf_len[k], n - 1);
   }
-  // ---- doomed bad cells of a VC (vcDoomedBadCells, hived_algorithm.go:80)
+  // ---- doomed bad cells of a VC (vcDoomedBadCells, hived_algorithm.go:80).  The reference's list is a slice and
+  // releaseBadCell (hived_algorithm.go:1487-1500) unbinds a doomed bad cell below a released bad preassigned cell without
+  // taking it off its VC's list: a list can hold stale (unbound) entries, more entries than the VC has preassigned cells
+  // of the level, and a cell more than once or in several VCs' lists.  p_dmcnt counts a cell's entries over all lists
+  // (0 answers the common case in O(1)); otherwise the short segment is searched for the FIRST occurrence, as
+  // listContains / listRemove (types.go:69-95) do.
+  HIVED_DEV int dm_find(int k, int cell) const {
+    const int32_t* a = d.dm_data + d.dm_base[k];
+    return firstIdx(d.dm_len[k], [&](int i) { return a[i] == cell; });
+  }
   HIVED_DEV void dm_append(int vc, int chain, int level, int cell) {
     int k = vcl(vc, chain, level);
     int n = d.dm_len[k];
-    if (n >= d.dm_cap[k]) { panic(HIVED_ERR_PLATFORM); return; }
+    if (n >= d.dm_cap[k]) { panic(HIVED_ERR_CAPACITY); return; }  // more stale entries than DM_STALE_SLACK (hived_topo.hpp)
+    const int cnt = d.p_dmcnt[cell];
     hv_warp_sync();
     ST(d.dm_data[d.dm_base[k] + n], cell);
-    ST(d.p_dmpos[cell], n);
-    ST(d.p_dmvc[cell], vc);
+    ST(d.p_dmcnt[cell], cnt + 1);
     ST(d.dm_len[k], n + 1);
   }
   HIVED_DEV void dm_remove(int vc, int chain, int level, int cell) {
     int k = vcl(vc, chain, level);
-    int pos = d.p_dmpos[cell];
-    if (pos < 0 || d.p_dmvc[cell] != vc) { panic(HIVED_ERR_PLATFORM); return; }
+    const int cnt = d.p_dmcnt[cell];
+    int pos = cnt > 0 ? dm_find(k, cell) : -1;
+    if (pos < 0) { panic(HIVED_ERR_PLATFORM); return; }  // "Cell not not found in list when removing"
     int n = d.dm_len[k];
     int last = d.dm_data[d.dm_base[k] + n - 1];
     hv_warp_sync();
     ST(d.dm_data[d.dm_base[k] + pos], last);
-    ST(d.p_dmpos[last], pos);
-    ST(d.p_dmpos[cell], -1);
-    ST(d.p_dmvc[cell], -1);
+    ST(d.p_dmcnt[cell], cnt - 1);
     ST(d.dm_len[k], n - 1);
   }
-  HIVED_DEV bool dm_contains(int vc, int cell) const { return d.p_dmpos[cell] >= 0 && d.p_dmvc[cell] == vc; }
+  HIVED_DEV bool dm_contains(int vc, int cell) const {
+    return d.p_dmcnt[cell] > 0 && dm_find(vcl(vc, d.p_chain[cell], d.p_level[cell]), cell) >= 0;
+  }
 
   // ======================================================================================
   // cell primitives

@@ -55,7 +55,7 @@ struct GroupMemFld {  // indexed by g * 8 + m like the flat arrays it replaces
 #define HIVED_MUTABLE_ARRAYS(Y)                                                                        \
   Y(p_prio, S.NP, -2) Y(p_state, S.NP, 0) Y(p_healthy, S.NP, 1) Y(p_vcell, S.NP, -1) Y(p_split, S.NP, 0) \
   Y(p_using, S.NP, -1) Y(p_resv, S.NP, -1) Y(p_usedopp, S.NP, 0) Y(p_flpos, S.NP, -1)                  \
-  Y(p_bfpos, S.NP, -1) Y(p_dmpos, S.NP, -1) Y(p_dmvc, S.NP, -1)                                        \
+  Y(p_bfpos, S.NP, -1) Y(p_dmcnt, S.NP, 0)                                                               \
   Y(v_prio, S.NV, -2) Y(v_state, S.NV, 0) Y(v_healthy, S.NV, 1) Y(v_pcell, S.NV, -1)                   \
   Y(vcFree, S.nVCs * S.nChains * MAXL, 0) Y(allVCFree, S.nChains * MAXL, 0)                            \
   Y(totalLeft, S.nChains * MAXL, 0) Y(allVCDoomed, S.nChains * MAXL, 0)                                \

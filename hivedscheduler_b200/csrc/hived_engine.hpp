@@ -435,7 +435,7 @@ struct Engine {
     std::vector<std::pair<void*, size_t>> v;
     const size_t NP = (size_t)dev.S.NP * 4, LV = (size_t)dev.S.nChains * MAXL * 4;
     v.push_back({dev.p_split, NP}); v.push_back({dev.p_flpos, NP}); v.push_back({dev.p_bfpos, NP});
-    v.push_back({dev.p_dmpos, NP}); v.push_back({dev.p_dmvc, NP});
+    v.push_back({dev.p_dmcnt, NP});
     v.push_back({dev.vcFree, LV * dev.S.nVCs}); v.push_back({dev.allVCFree, LV}); v.push_back({dev.totalLeft, LV});
     v.push_back({dev.allVCDoomed, LV});
     v.push_back({dev.fl_data, (size_t)dev.S.flTotal * 4}); v.push_back({dev.fl_len, LV}); v.push_back({dev.fl_dup, LV});
@@ -1007,6 +1007,63 @@ uint64_t hived_debug_view_hash(hived_ctx* ctx) {
       h ^= 0xff; h *= HIVED_FNV_PRIME;
     }
     total += h;
+  }
+  return total;
+}
+/* test hook: a hash of the state that decides future picks without showing in any result — per (chain, level)
+   totalLeft, allVCFree, allVCDoomed and the free and bad-free lists in list order, per (VC, chain, level) vcFree and
+   the doomed-bad list in list order (duplicates and stale entries included).  Keyed by names and addresses; segments
+   are combined order-independently, an all-zero segment counts as absent.  oracle/oracle_abi.cpp has the same
+   definition. */
+uint64_t hived_debug_bookkeeping_hash(hived_ctx* ctx) {
+  using hived::MAXL;
+  hived::Engine& e = ctx->e;
+  const hived::FlatTopo& T = e.T;
+  const size_t LV = (size_t)T.nChains * MAXL;
+  std::vector<int32_t> vcFree, allVCFree, totalLeft, doomed, fl, flLen, bf, bfLen, dm, dmLen;
+  e.readArray(e.dev.vcFree, vcFree, LV * T.nVCs);
+  e.readArray(e.dev.allVCFree, allVCFree, LV);
+  e.readArray(e.dev.totalLeft, totalLeft, LV);
+  e.readArray(e.dev.allVCDoomed, doomed, LV);
+  e.readArray(e.dev.fl_data, fl, T.flTotal);
+  e.readArray(e.dev.fl_len, flLen, LV);
+  e.readArray(e.dev.bf_data, bf, T.flTotal);
+  e.readArray(e.dev.bf_len, bfLen, LV);
+  e.readArray(e.dev.dm_data, dm, T.dmTotal);
+  e.readArray(e.dev.dm_len, dmLen, LV * T.nVCs);
+  auto str = [](uint64_t& h, const std::string& s) {
+    for (char ch : s) { h ^= (uint8_t)ch; h *= HIVED_FNV_PRIME; }
+    h ^= 0xff; h *= HIVED_FNV_PRIME;
+  };
+  auto num = [](uint64_t& h, int32_t v) {
+    for (int i = 0; i < 4; i++) { h ^= (uint8_t)((uint32_t)v >> (8 * i)); h *= HIVED_FNV_PRIME; }
+  };
+  auto list = [&](uint64_t& h, const int32_t* a, int32_t n) {
+    num(h, n);
+    for (int32_t i = 0; i < n; i++) str(h, T.pAddr[a[i]]);
+  };
+  uint64_t total = 0;
+  for (int32_t c = 0; c < T.nChains; c++) {
+    for (int32_t l = 1; l < MAXL; l++) {
+      const size_t k = (size_t)c * MAXL + l;
+      if (totalLeft[k] || allVCFree[k] || doomed[k] || flLen[k] || bfLen[k]) {
+        uint64_t h = HIVED_FNV_OFFSET;
+        str(h, "chain"); str(h, T.chainNames[c]); num(h, l);
+        num(h, totalLeft[k]); num(h, allVCFree[k]); num(h, doomed[k]);
+        list(h, fl.data() + T.fl_base[k], flLen[k]);
+        list(h, bf.data() + T.fl_base[k], bfLen[k]);
+        total += h;
+      }
+      for (int32_t v = 0; v < T.nVCs; v++) {
+        const size_t kv = (size_t)v * LV + k;
+        if (!vcFree[kv] && !dmLen[kv]) continue;
+        uint64_t h = HIVED_FNV_OFFSET;
+        str(h, "vc"); str(h, T.vcNames[v]); str(h, T.chainNames[c]); num(h, l);
+        num(h, vcFree[kv]);
+        list(h, dm.data() + T.dm_base[kv], dmLen[kv]);
+        total += h;
+      }
+    }
   }
   return total;
 }

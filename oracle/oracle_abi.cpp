@@ -562,4 +562,98 @@ uint64_t hived_debug_view_hash(hived_ctx* ctx) {
   return total;
 }
 
+/* oracle-only test hook: the length of vcDoomedBadCells[vc][chain][level]; *preassigned = the VC's non-pinned
+   preassigned cells of that level, *stale = entries whose cell is not bound to a virtual cell */
+int32_t hived_oracle_doomed_bad_list(hived_ctx* ctx, const char* vc, const char* chain, int32_t level,
+                                     int32_t* preassigned, int32_t* stale) {
+  const HivedAlgorithm& H = *ctx->h;
+  *preassigned = 0;
+  *stale = 0;
+  auto sit = H.vcSchedulers.find(vc);
+  if (sit != H.vcSchedulers.end()) {
+    auto cit = sit->second->nonPinnedPreassignedCells.find(chain);
+    if (cit != sit->second->nonPinnedPreassignedCells.end()) *preassigned = (int32_t)cit->second.at(level).size();
+  }
+  auto vit = H.vcDoomedBadCells.find(vc);
+  if (vit == H.vcDoomedBadCells.end()) return 0;
+  auto cit = vit->second.find(chain);
+  if (cit == vit->second.end()) return 0;
+  const CellList& l = cit->second.at(level);
+  for (const Cell* c : l) *stale += c->virtualCell == nullptr;
+  return (int32_t)l.size();
+}
+
+/* test hook (same definition as the device library's): per (chain, level) totalLeftCellNum, allVCFreeCellNum,
+   allVCDoomedBadCellNum, freeCellList and badFreeCells in list order; per (VC, chain, level) vcFreeCellNum and
+   vcDoomedBadCells in list order.  An all-zero segment counts as absent (a missing map entry is a zero). */
+uint64_t hived_debug_bookkeeping_hash(hived_ctx* ctx) {
+  const HivedAlgorithm& H = *ctx->h;
+  auto str = [](uint64_t& h, const std::string& s) {
+    for (char ch : s) { h ^= (uint8_t)ch; h *= HIVED_FNV_PRIME; }
+    h ^= 0xff; h *= HIVED_FNV_PRIME;
+  };
+  auto num = [](uint64_t& h, int32_t v) {
+    for (int i = 0; i < 4; i++) { h ^= (uint8_t)((uint32_t)v >> (8 * i)); h *= HIVED_FNV_PRIME; }
+  };
+  auto list = [&](uint64_t& h, const CellList& a) {
+    num(h, (int32_t)a.size());
+    for (const Cell* c : a) str(h, c->address);
+  };
+  auto count = [](const auto& m, const std::string& chain, int32_t l) -> int32_t {
+    auto it = m.find(chain);
+    if (it == m.end()) return 0;
+    auto jt = it->second.find(l);
+    return jt == it->second.end() ? 0 : jt->second;
+  };
+  static const CellList empty;
+  auto cells = [](const std::map<std::string, ChainCellList>& m, const std::string& chain, int32_t l) -> const CellList& {
+    auto it = m.find(chain);
+    return it == m.end() ? empty : it->second.at(l);
+  };
+  // every (chain, level) any of the maps knows
+  std::map<std::string, std::set<int32_t>> keys;
+  for (auto* m : {&H.allVCFreeCellNum, &H.totalLeftCellNum, &H.allVCDoomedBadCellNum})
+    for (auto& kv : *m) for (auto& lv : kv.second) keys[kv.first].insert(lv.first);
+  for (auto* m : {&H.freeCellList, &H.badFreeCells})
+    for (auto& kv : *m) for (auto& lv : kv.second.m) keys[kv.first].insert(lv.first);
+  for (auto& vk : H.vcFreeCellNum)
+    for (auto& kv : vk.second) for (auto& lv : kv.second) keys[kv.first].insert(lv.first);
+  for (auto& vk : H.vcDoomedBadCells)
+    for (auto& kv : vk.second) for (auto& lv : kv.second.m) keys[kv.first].insert(lv.first);
+  std::set<std::string> vcs;
+  for (auto& vk : H.vcFreeCellNum) vcs.insert(vk.first);
+  for (auto& vk : H.vcDoomedBadCells) vcs.insert(vk.first);
+  uint64_t total = 0;
+  for (auto& ck : keys) {
+    const std::string& chain = ck.first;
+    for (int32_t l : ck.second) {
+      const int32_t left = count(H.totalLeftCellNum, chain, l), free = count(H.allVCFreeCellNum, chain, l);
+      const int32_t doomed = count(H.allVCDoomedBadCellNum, chain, l);
+      const CellList& fl = cells(H.freeCellList, chain, l);
+      const CellList& bf = cells(H.badFreeCells, chain, l);
+      if (left || free || doomed || !fl.empty() || !bf.empty()) {
+        uint64_t h = HIVED_FNV_OFFSET;
+        str(h, "chain"); str(h, chain); num(h, l);
+        num(h, left); num(h, free); num(h, doomed);
+        list(h, fl);
+        list(h, bf);
+        total += h;
+      }
+      for (const std::string& vc : vcs) {
+        auto fit = H.vcFreeCellNum.find(vc);
+        const int32_t vfree = fit == H.vcFreeCellNum.end() ? 0 : count(fit->second, chain, l);
+        auto dit = H.vcDoomedBadCells.find(vc);
+        const CellList& dm = dit == H.vcDoomedBadCells.end() ? empty : cells(dit->second, chain, l);
+        if (!vfree && dm.empty()) continue;
+        uint64_t h = HIVED_FNV_OFFSET;
+        str(h, "vc"); str(h, vc); str(h, chain); num(h, l);
+        num(h, vfree);
+        list(h, dm);
+        total += h;
+      }
+    }
+  }
+  return total;
+}
+
 }  // extern "C"

@@ -2,7 +2,9 @@
 """API-level parity fuzz: random Schedule / AddAllocatedPod / DeleteAllocatedPod / DeleteUnallocatedPod calls and node
 health flips on the reference's own test cluster (example/config/design, with its 46 pod specs), through the host
 mirror of internal.SchedulerAlgorithm, on two implementations of include/hived.h in lock step.  After EVERY call the
-results (bind info / victims / wait reason / error class) and every cell's state are compared.  A platform error
+results (bind info / victims / wait reason / error class), every cell's state, the order of every cluster view and the
+bookkeeping that decides future picks (free, bad-free and doomed-bad lists in list order, the free / left / doomed
+counters) are compared.  FUZZ_CLUSTER=synthetic runs the synthetic cluster instead of the design config.  A platform error
 (the reference's panic) ends a run on both sides — the reference leaves its state undefined there.
 
     python tests/fuzz_api.py emu  [first_seed n_seeds n_ops]   device program (1-lane host emulation) vs oracle
@@ -66,17 +68,23 @@ def synthetic_fixture():
     return {"design_config": cfg, "pss": pss}
 
 
+def env_fixture():
+    """The cluster and pod specs FUZZ_CLUSTER names: "synthetic" or (default) the reference's design config."""
+    return synthetic_fixture() if os.environ.get("FUZZ_CLUSTER") == "synthetic" else load_fixture()
+
+
 def run_seed(lib_a, lib_b, seed: int, n_ops: int, fx=None, verbose=False):
     """Returns None (no divergence) or a description of the first one."""
-    fx = fx or (synthetic_fixture() if os.environ.get("FUZZ_CLUSTER") == "synthetic" else load_fixture())
+    fx = fx or env_fixture()
     rng = random.Random(seed)
     cfg = new_config(copy.deepcopy(fx["design_config"]))
     hs = [alg.HivedAlgorithm(cfg, lib=lib, max_groups=1024, max_pods=4096, max_group_leaves=128, max_group_pods=16)
           for lib in (lib_a, lib_b)]
     import ctypes as C
     for lib in (lib_a, lib_b):
-        lib.hived_debug_view_hash.restype = C.c_uint64
-        lib.hived_debug_view_hash.argtypes = [C.c_void_p]
+        for hook in (lib.hived_debug_view_hash, lib.hived_debug_bookkeeping_hash):
+            hook.restype = C.c_uint64
+            hook.argtypes = [C.c_void_p]
     nodes = list(hs[0].node_names)
     healthy = {n: False for n in nodes}
     for n in nodes:
@@ -165,6 +173,10 @@ def run_seed(lib_a, lib_b, seed: int, n_ops: int, fx=None, verbose=False):
             va, vb = (int(h._lib.hived_debug_view_hash(h._ctx)) for h in hs)
             if va != vb:
                 return "seed %d op %d %s: the persisted order of a cluster view differs" % (seed, step, what)
+            ba, bb = (int(h._lib.hived_debug_bookkeeping_hash(h._ctx)) for h in hs)
+            if ba != bb:
+                return "seed %d op %d %s: bookkeeping differs (free / bad-free / doomed-bad lists or counters)" % (
+                    seed, step, what)
             if verbose:
                 print(step, what, ra if what.startswith("Schedule") else "")
     finally:
@@ -189,7 +201,7 @@ def main():
         os.makedirs(os.path.dirname(path), exist_ok=True)
         subprocess.check_call(["g++", "-O1", "-g", "-std=c++17", "-fPIC", "-shared", "-o", path, os.path.join(HERE, "emu", src)])
         lib = _cabi.load_library(path)
-    fx = load_fixture()
+    fx = env_fixture()
     bad = 0
     for seed in range(first, first + count):
         d = run_seed(lib, oracle, seed, n_ops, fx)
