@@ -111,6 +111,12 @@ struct Core {
 #else
   const Dev& d;
 #endif
+  // The lane index and the ancestor-table width are NOT members: Core lives in the thread's stack frame (its `this` goes
+  // to the out-of-line member functions), and the compiler cannot tell a store through a state pointer from a store
+  // into that frame, so a member is reloaded from local memory (LDL) after nearly every store on the leader's path.
+  // The lane comes from the thread index, the width from the constant bank (CUDA build).  (until the end of this header)
+#define lane hv_lane()
+#define AS d.S.AS
 #if defined(__CUDACC__) && !defined(HIVED_SIMT_EMU) && !defined(HIVED_EMU)
   // the CTA's shared block is ONE file-scope __shared__ object: every access compiles to LDS / STS / ATOMS (through a
   // generic Sm* the compiler loses the address space as soon as `this` goes through memory: LD.E / ATOM.E)
@@ -124,8 +130,6 @@ struct Core {
   long long pool_cap;
   long long poolOff;
   int panicCode;  // sticky platform-error code of the current event
-  const int lane;
-  const int AS;
   Scratch s;                // this CTA's private scratch arrays
   // ---- VC-parallel execution (several CTAs, one per group of VCs; see run())
   const int cta, nCta;
@@ -146,7 +150,7 @@ struct Core {
 #if !(defined(__CUDACC__) && !defined(HIVED_SIMT_EMU) && !defined(HIVED_EMU))
         sm_(s_),
 #endif
-        sugg(nullptr), pool(pool_), pool_cap(cap), poolOff(0), panicCode(0), lane(hv_lane()), AS(dev.S.AS),
+        sugg(nullptr), pool(pool_), pool_cap(cap), poolOff(0), panicCode(0),
         s(dev.scratch[hv_cta()]), cta(hv_cta()), nCta(nCta_), multi(nCta_ > 1), curEvent(0), sharedHeld(false), prioMask(0) {
     for (int i = 0; i < N_WORK; i++) work[i] = 0;
     for (int i = 0; i < PC_COUNT; i++) pathCnt[i] = 0;
@@ -3339,80 +3343,93 @@ struct Core {
     }
   }
 
+  // a worker warp: serves the leader's full view passes until it posts CMD_EXIT
+  HIVED_DEV void serveViewPasses() {
+    while (true) {
+      hv_cta_sync();
+      if (smp()->cmd == CMD_EXIT) break;
+      sugg = smp()->a_sugg;
+      viewOp();
+    }
+  }
+
   // the CTA's main loop: leader warp walks its share of the ordered batch, the other warps serve view
   // passes.  own[0..nOwn): ascending indices of the events this CTA owns (nullptr: all of them).
+  // The register split (hv_regs_lead_group) gives the leader's warpgroup the registers the parked workers do not use;
+  // each group's code is a separate branch down to the end, so the worker loop is there twice.
   HIVED_DEV void run(const hived_event_t* events, int n, hived_result_t* results, const uint32_t* suggPool, const int32_t* aux,
                      const int32_t* initLists, int nPinnedOrder, int nBad, const int32_t* own, int nOwn) {
-    if (hv_warp() == 0) {
-      poolOff = smp()->pool_off;
-      int initPanic = 0;
-      if (initLists) { initState(initLists, nPinnedOrder, initLists + nPinnedOrder, nBad); initPanic = panicCode; }
-      if (!own) nOwn = n;
-      // the CTA's event indices travel through a 64-entry window in shared memory, refilled 32 at a time (lane =
-      // entry): the index of the next event is never a dependent global load on the leader's path
-      if (own) { for (int q = lane; q < 64; q += HIVED_WARPSZ) { const int idx = mgStart + q; if (idx < nOwn) smp()->own_win[idx & 63] = own[idx]; } }
-      ST(smp()->bkc_sched, -1);
-      hv_warp_sync();
-      auto ownAt = [&](int kk) { return own ? smp()->own_win[kk & 63] : kk; };
-      int stopK = nOwn;
-      mgStop = false;
-      for (int k = mgStart; k < nOwn; k++) {
-        if (own && k > mgStart && (k & 31) == 0) {
-          for (int q = lane; q < 32; q += HIVED_WARPSZ) { const int idx = k + 32 + q; if (idx < nOwn) smp()->own_win[idx & 63] = own[idx]; }
-          hv_warp_sync();
-        }
-        int i = ownAt(k);
-        if (lane == 0) hv_publish_smem(&smp()->lead_k, k);
-        curEvent = i;
-        sharedHeld = false;
-        long long tq = pclock();
-        // The events are streamed from HBM once.  Event k was requested while event k-1 ran (asynchronous 16-byte
-        // copies into the other half of the double buffer: no register target, nothing waits at a call boundary);
-        // wait for it, then request event k+1 and pull event k+2 towards L2/L1.
-        constexpr int EVQ = (int)(sizeof(hived_event_t) / 16);
-        int32_t* cur = smp()->ev_words[k & 1];
-        if (k == mgStart) { for (int q = lane; q < EVQ; q += HIVED_WARPSZ) hv_cp_async16(cur + 4 * q, reinterpret_cast<const char*>(&events[i]) + 16 * q); }
-        hv_cp_async_wait();
-        hv_warp_sync();
-        if (k + 1 < nOwn) {
-          const char* nxt = reinterpret_cast<const char*>(&events[ownAt(k + 1)]);
-          int32_t* dst = smp()->ev_words[(k + 1) & 1];
-          for (int q = lane; q < EVQ; q += HIVED_WARPSZ) hv_cp_async16(dst + 4 * q, nxt + 16 * q);
-        }
-        if (k + 2 < nOwn) hv_prefetch(&events[ownAt(k + 2)]);
-        dbg(14, tq);
-        processEvent(*reinterpret_cast<const hived_event_t*>(cur), &results[i], suggPool, aux);
-        if (mgStop) { hv_cp_async_wait(); stopK = k; break; }
-        tq = pclock();
-        if (multi) {
-          int next = (k + 1 < nOwn) ? ownAt(k + 1) : 0x7fffffff;
-          // release: only an event that touched the cluster-wide state publishes anything another CTA may read
-          // (free lists, counters, and the cells it put into them — with everything this CTA wrote to those
-          // cells in earlier events, the fence being cumulative).  Other events move the progress word on with a
-          // plain store: the fence (MEMBAR + L1 invalidation) after every event kept the L1 cold.
-          if (sharedHeld) hv_fence();
-          if (lane == 0) hv_st_volatile(d.progress + cta, next);
-          hv_warp_sync();
-        }
-        dbg(15, tq);
-      }
-      if (lane == 0) hv_publish_smem(&smp()->lead_k, 0x7fffffff);
-      flushWork();
-      ST(smp()->pool_off, poolOff);
-      ST(smp()->stop_k, stopK);
-      ST(smp()->panic, initPanic);
-      ST(smp()->cmd, CMD_EXIT);
-      hv_cta_sync();
-    } else if (hv_is_runahead()) {
-      if (!initLists) runAhead(events, n, own, nOwn);
+    if (hv_in_lead_group()) {
+      hv_regs_lead_group();
+      if (hv_warp() == 0) runLeader(events, n, results, suggPool, aux, initLists, nPinnedOrder, nBad, own, nOwn);
+      else serveViewPasses();
     } else {
-      while (true) {
-        hv_cta_sync();
-        if (smp()->cmd == CMD_EXIT) break;
-        sugg = smp()->a_sugg;
-        viewOp();
-      }
+      hv_regs_other_group();
+      if (!hv_is_runahead()) serveViewPasses();
+      else if (!initLists) runAhead(events, n, own, nOwn);
     }
+  }
+  HIVED_DEV void runLeader(const hived_event_t* events, int n, hived_result_t* results, const uint32_t* suggPool, const int32_t* aux,
+                           const int32_t* initLists, int nPinnedOrder, int nBad, const int32_t* own, int nOwn) {
+    poolOff = smp()->pool_off;
+    int initPanic = 0;
+    if (initLists) { initState(initLists, nPinnedOrder, initLists + nPinnedOrder, nBad); initPanic = panicCode; }
+    if (!own) nOwn = n;
+    // the CTA's event indices travel through a 64-entry window in shared memory, refilled 32 at a time (lane =
+    // entry): the index of the next event is never a dependent global load on the leader's path
+    if (own) { for (int q = lane; q < 64; q += HIVED_WARPSZ) { const int idx = mgStart + q; if (idx < nOwn) smp()->own_win[idx & 63] = own[idx]; } }
+    ST(smp()->bkc_sched, -1);
+    hv_warp_sync();
+    auto ownAt = [&](int kk) { return own ? smp()->own_win[kk & 63] : kk; };
+    int stopK = nOwn;
+    mgStop = false;
+    for (int k = mgStart; k < nOwn; k++) {
+      if (own && k > mgStart && (k & 31) == 0) {
+        for (int q = lane; q < 32; q += HIVED_WARPSZ) { const int idx = k + 32 + q; if (idx < nOwn) smp()->own_win[idx & 63] = own[idx]; }
+        hv_warp_sync();
+      }
+      int i = ownAt(k);
+      if (lane == 0) hv_publish_smem(&smp()->lead_k, k);
+      curEvent = i;
+      sharedHeld = false;
+      long long tq = pclock();
+      // The events are streamed from HBM once.  Event k was requested while event k-1 ran (asynchronous 16-byte
+      // copies into the other half of the double buffer: no register target, nothing waits at a call boundary);
+      // wait for it, then request event k+1 and pull event k+2 towards L2/L1.
+      constexpr int EVQ = (int)(sizeof(hived_event_t) / 16);
+      int32_t* cur = smp()->ev_words[k & 1];
+      if (k == mgStart) { for (int q = lane; q < EVQ; q += HIVED_WARPSZ) hv_cp_async16(cur + 4 * q, reinterpret_cast<const char*>(&events[i]) + 16 * q); }
+      hv_cp_async_wait();
+      hv_warp_sync();
+      if (k + 1 < nOwn) {
+        const char* nxt = reinterpret_cast<const char*>(&events[ownAt(k + 1)]);
+        int32_t* dst = smp()->ev_words[(k + 1) & 1];
+        for (int q = lane; q < EVQ; q += HIVED_WARPSZ) hv_cp_async16(dst + 4 * q, nxt + 16 * q);
+      }
+      if (k + 2 < nOwn) hv_prefetch(&events[ownAt(k + 2)]);
+      dbg(14, tq);
+      processEvent(*reinterpret_cast<const hived_event_t*>(cur), &results[i], suggPool, aux);
+      if (mgStop) { hv_cp_async_wait(); stopK = k; break; }
+      tq = pclock();
+      if (multi) {
+        int next = (k + 1 < nOwn) ? ownAt(k + 1) : 0x7fffffff;
+        // release: only an event that touched the cluster-wide state publishes anything another CTA may read
+        // (free lists, counters, and the cells it put into them — with everything this CTA wrote to those
+        // cells in earlier events, the fence being cumulative).  Other events move the progress word on with a
+        // plain store: the fence (MEMBAR + L1 invalidation) after every event kept the L1 cold.
+        if (sharedHeld) hv_fence();
+        if (lane == 0) hv_st_volatile(d.progress + cta, next);
+        hv_warp_sync();
+      }
+      dbg(15, tq);
+    }
+    if (lane == 0) hv_publish_smem(&smp()->lead_k, 0x7fffffff);
+    flushWork();
+    ST(smp()->pool_off, poolOff);
+    ST(smp()->stop_k, stopK);
+    ST(smp()->panic, initPanic);
+    ST(smp()->cmd, CMD_EXIT);
+    hv_cta_sync();
   }
 
 #if defined(__CUDACC__) && !defined(HIVED_EMU)
@@ -3425,70 +3442,69 @@ struct Core {
   HIVED_DEV void serve(volatile int32_t* slot, int seq0, int idleSpins, hived_result_t* stageRes, uint32_t* dSugg, int32_t* dAux,
                        int nPinnedOrder, int nBad) {
     (void)nPinnedOrder; (void)nBad;
-    if (hv_warp() == 0) {
-      int lastSeq = seq0;
-      ST(smp()->bkc_sched, -1);
-      while (true) {
-        int seq = lastSeq, spins = 0;
-        // header line: [0] seq  [1] n (0 = STOP)  [2] suggWords  [3] auxWords  [4] poolCap
-        int hdr = 0;
-        while (true) {
-          hdr = lane < 8 ? slot[lane] : 0;
-          seq = hv_shfl(hdr, 0);
-          if (seq != lastSeq) break;
-          if (++spins > idleSpins) break;
-        }
-        if (seq == lastSeq) break;  // idle: leave
-        const int n = hv_shfl(hdr, 1), suggWords = hv_shfl(hdr, 2), auxWords = hv_shfl(hdr, 3);
-        pool_cap = hv_shfl(hdr, 4);
-        lastSeq = seq;
-        if (n <= 0) break;  // STOP
-        // payload: events at word SERVE_EV_OFF, then the suggested bitmaps, then aux
-        const volatile int32_t* pay = slot + SERVE_EV_OFF;
-        const int evWords = (int)(sizeof(hived_event_t) / 4);
-        const volatile int32_t* hs = pay + SERVE_MAX_EVENTS * evWords;
-        for (int i = lane; i < suggWords; i += HIVED_WARPSZ) dSugg[i] = (uint32_t)hs[i];
-        const volatile int32_t* ha = hs + suggWords;
-        for (int i = lane; i < auxWords; i += HIVED_WARPSZ) dAux[i] = ha[i];
-        hv_warp_sync();
-        poolOff = 0;
-        for (int k = 0; k < n; k++) {
-          int32_t* cur = smp()->ev_words[k & 1];
-          for (int i = lane; i < evWords; i += HIVED_WARPSZ) cur[i] = pay[k * evWords + i];
-          hv_warp_sync();
-          curEvent = k;
-          sharedHeld = false;
-          processEvent(*reinterpret_cast<const hived_event_t*>(cur), &stageRes[k], suggWords > 0 ? dSugg : nullptr, auxWords > 0 ? dAux : nullptr);
-        }
-        flushWork();
-        hv_warp_sync();
-        // response: results at SERVE_RES_OFF, pool window after them, then [poolOff, panic]; `done` last
-        volatile int32_t* out = slot + SERVE_RES_OFF;
-        const int32_t* sr = reinterpret_cast<const int32_t*>(stageRes);
-        const int resWords = n * (int)(sizeof(hived_result_t) / 4);
-        for (int i = lane; i < resWords; i += HIVED_WARPSZ) out[i] = sr[i];
-        volatile int32_t* op = out + SERVE_MAX_EVENTS * (int)(sizeof(hived_result_t) / 4);
-        const long long used = poolOff < SERVE_POOL_WINDOW ? poolOff : SERVE_POOL_WINDOW;
-        for (int i = lane; i < (int)used; i += HIVED_WARPSZ) op[i] = pool[i];
-        if (lane == 0) { slot[SERVE_DONE_OFF + 1] = (int32_t)poolOff; slot[SERVE_DONE_OFF + 2] = (int32_t)(poolOff >> 32); }
-        __threadfence_system();
-        hv_warp_sync();
-        if (lane == 0) slot[SERVE_DONE_OFF] = seq;
-        hv_warp_sync();
-      }
-      ST(smp()->cmd, CMD_EXIT);
-      hv_cta_sync();
-      if (lane == 0) { __threadfence_system(); slot[SERVE_DONE_OFF + 3] = lastSeq; slot[SERVE_DONE_OFF + 4] = 1; }  // exited
-    } else if (hv_is_runahead()) {
-      return;
+    if (hv_in_lead_group()) {  // (the register split of run())
+      hv_regs_lead_group();
+      if (hv_warp() == 0) serveLeader(slot, seq0, idleSpins, stageRes, dSugg, dAux);
+      else serveViewPasses();
     } else {
-      while (true) {
-        hv_cta_sync();
-        if (smp()->cmd == CMD_EXIT) break;
-        sugg = smp()->a_sugg;
-        viewOp();
-      }
+      hv_regs_other_group();
+      if (!hv_is_runahead()) serveViewPasses();
     }
+  }
+  HIVED_DEV void serveLeader(volatile int32_t* slot, int seq0, int idleSpins, hived_result_t* stageRes, uint32_t* dSugg, int32_t* dAux) {
+    int lastSeq = seq0;
+    ST(smp()->bkc_sched, -1);
+    while (true) {
+      int seq = lastSeq, spins = 0;
+      // header line: [0] seq  [1] n (0 = STOP)  [2] suggWords  [3] auxWords  [4] poolCap
+      int hdr = 0;
+      while (true) {
+        hdr = lane < 8 ? slot[lane] : 0;
+        seq = hv_shfl(hdr, 0);
+        if (seq != lastSeq) break;
+        if (++spins > idleSpins) break;
+      }
+      if (seq == lastSeq) break;  // idle: leave
+      const int n = hv_shfl(hdr, 1), suggWords = hv_shfl(hdr, 2), auxWords = hv_shfl(hdr, 3);
+      pool_cap = hv_shfl(hdr, 4);
+      lastSeq = seq;
+      if (n <= 0) break;  // STOP
+      // payload: events at word SERVE_EV_OFF, then the suggested bitmaps, then aux
+      const volatile int32_t* pay = slot + SERVE_EV_OFF;
+      const int evWords = (int)(sizeof(hived_event_t) / 4);
+      const volatile int32_t* hs = pay + SERVE_MAX_EVENTS * evWords;
+      for (int i = lane; i < suggWords; i += HIVED_WARPSZ) dSugg[i] = (uint32_t)hs[i];
+      const volatile int32_t* ha = hs + suggWords;
+      for (int i = lane; i < auxWords; i += HIVED_WARPSZ) dAux[i] = ha[i];
+      hv_warp_sync();
+      poolOff = 0;
+      for (int k = 0; k < n; k++) {
+        int32_t* cur = smp()->ev_words[k & 1];
+        for (int i = lane; i < evWords; i += HIVED_WARPSZ) cur[i] = pay[k * evWords + i];
+        hv_warp_sync();
+        curEvent = k;
+        sharedHeld = false;
+        processEvent(*reinterpret_cast<const hived_event_t*>(cur), &stageRes[k], suggWords > 0 ? dSugg : nullptr, auxWords > 0 ? dAux : nullptr);
+      }
+      flushWork();
+      hv_warp_sync();
+      // response: results at SERVE_RES_OFF, pool window after them, then [poolOff, panic]; `done` last
+      volatile int32_t* out = slot + SERVE_RES_OFF;
+      const int32_t* sr = reinterpret_cast<const int32_t*>(stageRes);
+      const int resWords = n * (int)(sizeof(hived_result_t) / 4);
+      for (int i = lane; i < resWords; i += HIVED_WARPSZ) out[i] = sr[i];
+      volatile int32_t* op = out + SERVE_MAX_EVENTS * (int)(sizeof(hived_result_t) / 4);
+      const long long used = poolOff < SERVE_POOL_WINDOW ? poolOff : SERVE_POOL_WINDOW;
+      for (int i = lane; i < (int)used; i += HIVED_WARPSZ) op[i] = pool[i];
+      if (lane == 0) { slot[SERVE_DONE_OFF + 1] = (int32_t)poolOff; slot[SERVE_DONE_OFF + 2] = (int32_t)(poolOff >> 32); }
+      __threadfence_system();
+      hv_warp_sync();
+      if (lane == 0) slot[SERVE_DONE_OFF] = seq;
+      hv_warp_sync();
+    }
+    ST(smp()->cmd, CMD_EXIT);
+    hv_cta_sync();
+    if (lane == 0) { __threadfence_system(); slot[SERVE_DONE_OFF + 3] = lastSeq; slot[SERVE_DONE_OFF + 4] = 1; }  // exited
   }
 #endif
 };
@@ -3496,5 +3512,7 @@ struct Core {
 #ifdef HIVED_DEV_IN_CONSTANT
 #undef d
 #endif
+#undef lane
+#undef AS
 
 }  // namespace hived

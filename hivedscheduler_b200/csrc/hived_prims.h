@@ -23,6 +23,9 @@ inline int hv_nth() { return 1; }
 inline int hv_warp() { return 0; }
 inline int hv_nwarps() { return 1; }
 inline bool hv_is_runahead() { return false; }
+inline bool hv_in_lead_group() { return true; }
+inline void hv_regs_lead_group() {}
+inline void hv_regs_other_group() {}
 inline void hv_nanosleep() {}
 inline void hv_touch(const void*) {}
 inline void hv_cta_sync() {}
@@ -90,6 +93,10 @@ inline int hv_nth() { return simt::nth() - (hv_has_runahead() ? 32 : 0); }
 inline int hv_warp() { return simt::warp(); }
 inline int hv_nwarps() { return hv_nth() / 32; }
 inline bool hv_is_runahead() { return hv_has_runahead() && simt::warp() == hv_nwarps(); }
+// the roles of the CUDA build's register split (below); the reallocation itself has no host counterpart
+inline bool hv_in_lead_group() { return simt::warp() < 4 && !hv_is_runahead(); }
+inline void hv_regs_lead_group() {}
+inline void hv_regs_other_group() {}
 inline void hv_nanosleep() { simt::yield_to_scheduler(); }
 inline void hv_touch(const void* p) { (void)*(const volatile char*)p; }
 inline void hv_cta_sync() { simt::cta_barrier_n(hv_nth()); }
@@ -172,6 +179,16 @@ __device__ __forceinline__ int hv_nth() { return blockDim.x - 32; }
 __device__ __forceinline__ int hv_warp() { return threadIdx.x >> 5; }
 __device__ __forceinline__ int hv_nwarps() { return (blockDim.x >> 5) - 1; }
 __device__ __forceinline__ bool hv_is_runahead() { return (threadIdx.x >> 5) == (blockDim.x >> 5) - 1; }
+// Register split between the warpgroups of the 512-thread CTA (setmaxnreg, sm_90a).  __launch_bounds__(512, 1) caps
+// every thread at 128 registers, yet only the leader warp runs the long sequential code.  Warpgroup 0 (the leader and
+// workers 1-3) grows to HV_REGS_LEAD, warpgroups 1-3 (the other workers and the run-ahead warp) shrink to
+// HV_REGS_OTHER: 128 x 240 + 384 x 88 = 64 512 of the SM's 65 536.  The instruction is warpgroup-collective (all four
+// warps execute the same one).  ptxas compiles code that both groups reach under the smaller limit, so each group's
+// roles stay in a branch of their own until they are done (Core::run / Core::serve).
+constexpr int HV_REGS_LEAD = 240, HV_REGS_OTHER = 88;
+__device__ __forceinline__ bool hv_in_lead_group() { return threadIdx.x < 128; }
+__device__ __forceinline__ void hv_regs_lead_group() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(HV_REGS_LEAD)); }
+__device__ __forceinline__ void hv_regs_other_group() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(HV_REGS_OTHER)); }
 __device__ __forceinline__ void hv_nanosleep() { __nanosleep(200); }
 // pull a line towards L1 without a register target
 __device__ __forceinline__ void hv_touch(const void* p) {
