@@ -166,7 +166,7 @@ inline FlatTopo buildTopo(const std::string& text) {
     const Elem c = el[it->second.child];
     Elem e; e.level = c.level + 1; e.child = it->second.child; e.childNumber = it->second.n;
     e.hasNode = c.hasNode || it->second.node; e.isMultiNodes = c.hasNode; e.leafType = c.leafType; e.leafNum = c.leafNum * it->second.n;
-    if (e.level >= MAXL) throw TopoError("cell chain deeper than MAXL levels");
+    if (e.level >= MAXL) throw TopoError("a cell chain has more than MAXL - 1 levels", 102);
     el[ct] = e;
   };
   for (auto& kv : types) addChain(kv.first);

@@ -73,12 +73,14 @@ def env_fixture():
     return synthetic_fixture() if os.environ.get("FUZZ_CLUSTER") == "synthetic" else load_fixture()
 
 
-def run_seed(lib_a, lib_b, seed: int, n_ops: int, fx=None, verbose=False):
-    """Returns None (no divergence) or a description of the first one."""
+def run_seed(lib_a, lib_b, seed: int, n_ops: int, fx=None, verbose=False, max_group_leaves=128, max_group_pods=16):
+    """Returns None (no divergence) or a description of the first one.  max_group_leaves / max_group_pods: the
+    hived_options_t limits of both contexts (clusters with wide nodes or large gangs raise them)."""
     fx = fx or env_fixture()
     rng = random.Random(seed)
     cfg = new_config(copy.deepcopy(fx["design_config"]))
-    hs = [alg.HivedAlgorithm(cfg, lib=lib, max_groups=1024, max_pods=4096, max_group_leaves=128, max_group_pods=16)
+    hs = [alg.HivedAlgorithm(cfg, lib=lib, max_groups=1024, max_pods=4096, max_group_leaves=max_group_leaves,
+                             max_group_pods=max_group_pods)
           for lib in (lib_a, lib_b)]
     import ctypes as C
     for lib in (lib_a, lib_b):
