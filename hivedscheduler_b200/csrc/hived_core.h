@@ -2269,7 +2269,6 @@ struct Core {
   HIVED_DEV void deleteAllocatedAffinityGroup(int g) {
     int nl = groupLeaves(g);
     int vc = d.g_vc[g];
-    if (mgMode == 1 && mgDeleteNeedsShared(g, nl)) { mgStop = true; return; }
     if (leanDelete(g, nl, vc)) { eraseGroup(g); return; }
     path_add(PC_GENERAL_DELETE);
     if (deleteGroupBatched(g, nl, vc)) { eraseGroup(g); return; }
@@ -2524,7 +2523,7 @@ struct Core {
       reason = 0; rcell = -1;
       return true;
     }
-    if (mgMode == 1) { mgStop = true; return false; }  // the mapping may bind a preassigned cell (free lists)
+    if (mgMode == 1) { mgStopBeforeMapping(); return false; }  // the mapping may bind a preassigned cell (free lists)
     path_add(PC_GENERAL_MAP);
     tryLazyPreempt(s.pl_v, r.nleaves);
     if (panicCode) return false;
@@ -2573,7 +2572,7 @@ struct Core {
         vcHasType = true;
         r.chain = chain;
         if (handleSchedulingRequest(r, hasVirtual, reason, rcell)) { reason = 0; return 1; }
-        if (panicCode) return 0;
+        if (panicCode || mgStop) return 0;
       }
     }
     if (typeSpecified && r.priority >= 0 && !vcHasType) return -HIVED_ERR_LEAF_TYPE_NOT_IN_VC;
@@ -2604,7 +2603,9 @@ struct Core {
       int tr, tc;
       int rc = scheduleForLeafCellType(r, lt, false, hasVirtual, tr, tc);
       if (rc != 0) { reason = 0; rcell = -1; return rc; }
-      if (panicCode) return 0;
+      // a stopped attempt (multi-GPU partition) must not go on to the next chain: its fast placement would sort that
+      // chain's view now, which a sequential run does only when (and if) the event reaches it
+      if (panicCode || mgStop) return 0;
       if (tr != 0) { lastReason = tr; lastCell = tc; }
     }
     reason = lastReason; rcell = lastCell;
@@ -3077,6 +3078,9 @@ struct Core {
     int leafOff, podOff;
     memberOffsets(g, m, leafOff, podOff);
     const int occupant = gpods(g)[podOff + podIndex];
+    // multi-GPU partition: an event that stops is not written at all, so decide before the slot is cleared — the solo
+    // re-run must find the occupant there to report it
+    if (mgMode == 1 && mgDeleteStops(g, podOff + podIndex)) { mgStop = true; return; }
     ST(gpods(g)[podOff + podIndex], -1);
     ST(res->pod_index, occupant);
     const int32_t* po = gpods(g);

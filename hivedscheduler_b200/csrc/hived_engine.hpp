@@ -467,16 +467,26 @@ struct Engine {
     const int CL = C > 0 ? C : 1;
     std::vector<std::vector<int32_t>> lists(CL);
     std::vector<long long> need(CL, 0);
+    // a refused batch changes nothing: the group -> VC entries it wrote are put back
+    std::vector<std::pair<int, int32_t>> undo;
+    auto refuse = [&](int code, const char* why) {
+      for (auto it = undo.rbegin(); it != undo.rend(); ++it) groupVcHost[it->first] = it->second;
+      err = why;
+      return code;
+    };
     for (int i = 0; i < n; i++) {
       const hived_event_t& ev = events[i];
-      if (ev.type != HIVED_EV_SCHEDULE && ev.type != HIVED_EV_DELETE_ALLOCATED) { err = "multi-GPU partition: only SCHEDULE / DELETE_ALLOCATED events"; return HIVED_ERR_BAD_SPEC; }
+      if (ev.type != HIVED_EV_SCHEDULE && ev.type != HIVED_EV_DELETE_ALLOCATED) return refuse(HIVED_ERR_BAD_SPEC, "multi-GPU partition: only SCHEDULE / DELETE_ALLOCATED events");
+      // no rank holds a suggested-node pool: such an event would silently see every node as suggested
+      if (ev.suggested_off >= 0) return refuse(HIVED_ERR_BAD_SPEC, "multi-GPU partition: events with a suggested-node set are not supported");
       int evVc = ev.spec.vc;
       const int g = ev.spec.group;
       if (ev.type == HIVED_EV_SCHEDULE) {
         int p = ev.spec.priority;
         mask |= (p >= -1 && p < 62) ? (1ull << (p + 1)) : (1ull << 62);
         if (g >= 0 && g < (int)groupVcHost.size() && evVc >= 0 && evVc < T.nVCs) {
-          if (groupStamp[g] == batchStamp && groupVcHost[g] >= 0 && groupVcHost[g] != evVc) { err = "multi-GPU partition: a group id used under two VCs in one batch"; return HIVED_ERR_BAD_SPEC; }
+          if (groupStamp[g] == batchStamp && groupVcHost[g] >= 0 && groupVcHost[g] != evVc) return refuse(HIVED_ERR_BAD_SPEC, "multi-GPU partition: a group id used under two VCs in one batch");
+          undo.push_back({g, groupVcHost[g]});
           groupVcHost[g] = evVc;
           groupStamp[g] = batchStamp;
         }
@@ -485,7 +495,7 @@ struct Engine {
         evVc = (g >= 0 && g < (int)groupVcHost.size()) ? groupVcHost[g] : -1;
         if (evVc < 0) evVc = (ev.spec.vc >= 0 && ev.spec.vc < T.nVCs) ? ev.spec.vc : 0;
       }
-      if (evVc < 0 || evVc >= T.nVCs) { err = "multi-GPU partition: event with an unknown VC"; return HIVED_ERR_BAD_SPEC; }
+      if (evVc < 0 || evVc >= T.nVCs) return refuse(HIVED_ERR_BAD_SPEC, "multi-GPU partition: event with an unknown VC");
       if (evVc % world != rank) continue;
       const int c = evVc / world;
       lists[c].push_back(i);
@@ -495,15 +505,17 @@ struct Engine {
         need[c] += 3 * leaves;
       }
     }
+    if ((mask & (mask - 1)) != 0 || (mask & 1)) return refuse(HIVED_ERR_BAD_SPEC, "multi-GPU partition: more than one priority in use");
+    long long needAll = 0;
+    for (int c = 0; c < CL; c++) needAll += need[c];
+    if (needAll > poolCap) return refuse(HIVED_ERR_CAPACITY, "multi-GPU partition: pool too small");
     prioMaskHost = mask;
-    if ((mask & (mask - 1)) != 0 || (mask & 1)) { err = "multi-GPU partition: more than one priority in use"; return HIVED_ERR_BAD_SPEC; }
     launchCta = CL;
     ownOff.assign(CL + 1, 0);
     mgOwnHost.clear();
     for (int c = 0; c < CL; c++) { mgOwnHost.insert(mgOwnHost.end(), lists[c].begin(), lists[c].end()); ownOff[c + 1] = (int32_t)mgOwnHost.size(); }
     poolBase.assign(CL + 1, 0);
     for (int c = 0; c < CL; c++) poolBase[c + 1] = poolBase[c] + need[c];
-    if (poolBase[CL] > poolCap) { err = "multi-GPU partition: pool too small"; return HIVED_ERR_CAPACITY; }
     dOwn.ensure((size_t)(n + CL + 2) * 4);
     if (!mgOwnHost.empty()) bk_h2d(dOwn.p, mgOwnHost.data(), mgOwnHost.size() * 4);
     bk_h2d((int32_t*)dOwn.p + n, ownOff.data(), (size_t)(CL + 1) * 4);
@@ -981,8 +993,9 @@ int hived_bench_path_counters(hived_ctx* ctx, int64_t* out) {
   return hived::PC_COUNT;
 }
 /* test hook: a hash of every cluster view's persisted order (cell addresses in order; order-independent across views).
-   The order is state that no result shows until a tie is broken by it. */
-uint64_t hived_debug_view_hash(hived_ctx* ctx) {
+   The order is state that no result shows until a tie is broken by it.  vc >= 0: only the views of that VC (its
+   chain and pinned-cell schedulers, hived_debug_view_hash_vc). */
+static uint64_t viewHash(hived_ctx* ctx, int32_t vc) {
   hived::Engine& e = ctx->e;
   const hived::FlatTopo& T = e.T;
   std::vector<int32_t> cv, valid, head, cnt, next;
@@ -993,6 +1006,7 @@ uint64_t hived_debug_view_hash(hived_ctx* ctx) {
   e.readArray(e.dev.vn_next, next, T.NV);
   uint64_t total = 0;
   for (int s = 0; s < T.nScheds; s++) {
+    if (vc >= 0 && T.s_vc[s] != vc) continue;
     std::vector<int32_t> order;
     if (valid[s]) {
       for (int u = T.s_maxleaf[s]; u >= 0; u--)
@@ -1009,6 +1023,13 @@ uint64_t hived_debug_view_hash(hived_ctx* ctx) {
     total += h;
   }
   return total;
+}
+uint64_t hived_debug_view_hash(hived_ctx* ctx) { return viewHash(ctx, -1); }
+/* 0 for an unknown VC; oracle/oracle_abi.cpp has the same definition.  On a rank of a multi-GPU partition only the
+   views of its own VCs are current (include/hived_multigpu.h). */
+uint64_t hived_debug_view_hash_vc(hived_ctx* ctx, int32_t vc) {
+  if (vc < 0 || vc >= ctx->e.T.nVCs) return 0;
+  return viewHash(ctx, vc);
 }
 /* test hook: a hash of the state that decides future picks without showing in any result — per (chain, level)
    totalLeft, allVCFree, allVCDoomed and the free and bad-free lists in list order, per (VC, chain, level) vcFree and

@@ -31,8 +31,13 @@
  * touch the cluster-wide state: the sequential contract holds, results are identical to a single-GPU run (the
  * chain hash over the merged results — hived_mg_chain_hash — is the witness).  Only calm batches are accepted
  * (SCHEDULE / DELETE_ALLOCATED events, every node healthy, one guaranteed priority, no recovery): the regime in
- * which the single-GPU engine runs VC-parallel (hived_engine.hpp prepare()); anything else: HIVED_ERR_BAD_SPEC.
- * After the run a rank's physical-cell state is authoritative for its own VCs only.                              */
+ * which the single-GPU engine runs VC-parallel (hived_engine.hpp prepare()).  hived_mg_stage refuses with
+ * HIVED_ERR_BAD_SPEC, and changes nothing, a batch with any other event type, an event with a suggested-node set
+ * (suggested_off >= 0: no rank holds a suggested-node pool), more than one priority (or an opportunistic one), a
+ * group id scheduled under two VCs, or an event of an unknown VC; and any batch on a context with a bad node or a
+ * recovered pod.
+ * After the run a rank's physical-cell state and its views (hived_debug_view_hash_vc) are authoritative for its own
+ * VCs only.                                                                                                       */
 #ifndef HIVED_MULTIGPU_H_
 #define HIVED_MULTIGPU_H_
 #include "hived.h"

@@ -562,6 +562,27 @@ uint64_t hived_debug_view_hash(hived_ctx* ctx) {
   return total;
 }
 
+/* test hook (same definition as the device library's): hived_debug_view_hash restricted to the views of one VC (its
+   chain and pinned-cell schedulers); 0 for an unknown VC */
+uint64_t hived_debug_view_hash_vc(hived_ctx* ctx, int32_t vc) {
+  const HivedAlgorithm& H = *ctx->h;
+  if (vc < 0 || vc >= (int32_t)H.vcNames.size()) return 0;
+  auto it = H.vcSchedulers.find(H.vcNames[vc]);
+  if (it == H.vcSchedulers.end()) return 0;
+  uint64_t total = 0;
+  auto one = [&](const TopologyAwareScheduler* t) {
+    uint64_t h = HIVED_FNV_OFFSET;
+    for (const Node* n : t->cv) {
+      for (char ch : n->c->address) { h ^= (uint8_t)ch; h *= HIVED_FNV_PRIME; }
+      h ^= 0xff; h *= HIVED_FNV_PRIME;
+    }
+    total += h;
+  };
+  for (auto& s : it->second->nonPinnedCellSchedulers) one(s.second);
+  for (auto& s : it->second->pinnedCellSchedulers) one(s.second);
+  return total;
+}
+
 /* oracle-only test hook: the length of vcDoomedBadCells[vc][chain][level]; *preassigned = the VC's non-pinned
    preassigned cells of that level, *stale = entries whose cell is not bound to a virtual cell */
 int32_t hived_oracle_doomed_bad_list(hived_ctx* ctx, const char* vc, const char* chain, int32_t level,
