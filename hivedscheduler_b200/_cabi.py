@@ -124,6 +124,24 @@ SYMBOLS = [
     ("hived_result_hash", C.c_uint64, [_P]),
 ]
 
+HIVED_MANY_MAX = 16
+
+
+class Batch(C.Structure):
+    """hived_batch_t (include/hived_multictx.h)."""
+    _fields_ = [("ctx", _P), ("events", C.POINTER(Event)), ("n", C.c_int32),
+                ("suggested_pool", C.POINTER(C.c_uint32)), ("suggested_words", C.c_int64),
+                ("res", C.POINTER(Result)), ("pool", C.POINTER(C.c_int32)), ("pool_cap", C.c_int64),
+                ("rc", C.c_int32), ("reserved", C.c_int32), ("pool_used", C.c_int64)]
+
+
+def bind_many(lib: C.CDLL) -> C.CDLL:
+    """Type hived_process_events_many (include/hived_multictx.h) on a library loaded with load_library."""
+    lib.hived_process_events_many.restype = C.c_int
+    lib.hived_process_events_many.argtypes = [C.POINTER(Batch), C.c_int32]
+    return lib
+
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 CUDA_LIB_PATH = os.path.join(_HERE, "csrc", "libhived_cuda.so")
 

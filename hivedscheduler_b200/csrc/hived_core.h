@@ -30,6 +30,12 @@
 #include "hived_prims.h"
 
 namespace hived {
+#ifdef HIVED_MANY_BUILD
+// The second build of the program (hived_cuda_many.cu, joint launches of several contexts) lives in a namespace of its
+// own: the out-of-line members of Core would otherwise have the same names in both builds, and one copy would be
+// dropped at link time.
+namespace many {
+#endif
 
 #ifndef HIVED_TOPO_CONSTS
 constexpr int MAXL = 16;
@@ -90,7 +96,12 @@ __shared__ Sm g_hived_sm;  // one per CTA (both kernels of hived_cuda.cu use it)
 // on the leader warp's critical path and a third of its memory instructions.  One
 // context's Dev is loaded per device at a time; launchProgram / the per-call path reload it when the owner changes
 // (hived_cuda.cu: ensureDevLoaded).
+#ifdef HIVED_MANY_BUILD
+// Joint launches (include/hived_multictx.h): one Dev per listed context, CTA (x, y) is CTA x of context y.
+__constant__ Dev g_hived_devs[HIVED_MANY_MAX];
+#else
 __constant__ Dev g_hived_dev;
+#endif
 #define HIVED_DEV_IN_CONSTANT 1
 #endif
 
@@ -106,7 +117,9 @@ enum { CMD_IDLE = 0, CMD_VIEW = 1, CMD_EXIT = 2 };
 #endif
 
 struct Core {
-#ifdef HIVED_DEV_IN_CONSTANT
+#if defined(HIVED_DEV_IN_CONSTANT) && defined(HIVED_MANY_BUILD)
+#define d g_hived_devs[blockIdx.y]  /* (until the end of this header) */
+#elif defined(HIVED_DEV_IN_CONSTANT)
 #define d g_hived_dev  /* (until the end of this header) */
 #else
   const Dev& d;
@@ -3519,4 +3532,7 @@ struct Core {
 #undef lane
 #undef AS
 
+#ifdef HIVED_MANY_BUILD
+}  // namespace many
+#endif
 }  // namespace hived

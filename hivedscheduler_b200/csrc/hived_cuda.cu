@@ -12,7 +12,9 @@
 
 #include <mutex>
 
+#define HIVED_BK_LAUNCH_MANY 1  // the joint launch below
 #include "hived_engine.hpp"
+#include "hived_many.h"
 
 namespace hived {
 
@@ -271,6 +273,77 @@ int launchProgram(Engine& e, int n, bool withInit) {
   if (mgMode) { e.mgStopOut.assign(C, 0); for (int c = 0; c < C; c++) e.mgStopOut[c] = (int32_t)scal[c * 4 + 3]; }
   e.poolOff = scal[0];
   if (withInit && scal[2]) { e.err = "initialisation panicked on the device"; return (int)scal[2]; }
+  return 0;
+}
+
+// ---- joint launches (include/hived_multictx.h, hived_cuda_many.cu) ------------------------------------------------
+// The staged batches of several contexts of one device run in one launch, each context on CTAs of its own, on the first
+// context's stream.  g_hived_dev and its owner are not touched; but every resident per-call kernel of the device is
+// stopped first — the participants' (they would write the same state) and the owner's (it holds an SM the joint launch
+// may need to have all its CTAs resident).  Contexts whose CTAs do not fit on the device together go to further
+// launches (rounds), greedily in list order.
+int bk_launch_many(Engine* const* es, int k) {
+  std::lock_guard<std::recursive_mutex> lk(g_devMu);
+  Engine& e0 = *es[0];
+  const int dv = e0.deviceOrdinal >= 0 && e0.deviceOrdinal < 64 ? e0.deviceOrdinal : 0;
+  for (int y = 0; y < k; y++) bk_quiesce(*es[y]);
+  if (g_devOwner[dv]) bk_quiesce(*g_devOwner[dv]);
+  auto fail = [&](const std::string& why) {
+    for (int y = 0; y < k; y++) es[y]->err = why;
+    return HIVED_ERR_PLATFORM;
+  };
+  std::string err;
+  if (takeCopyError(err)) return fail(err);  // a staging copy of one of the batches failed
+  const int fit = manyCoResident(e0.deviceOrdinal);
+  if (fit <= 0) return fail("joint launch: cannot query the co-resident CTA limit");
+  CudaTimers* t = (CudaTimers*)e0.stream;
+  std::vector<long long> scal((size_t)k * MAX_CTAS * 4, 0);
+  ManyArgs a;
+  const Dev* devs[HIVED_MANY_MAX];
+  for (int y = 0; y < k; y++) {
+    Engine& e = *es[y];
+    const int C = e.launchCta;
+    long long* s = &scal[(size_t)y * MAX_CTAS * 4];
+    for (int c = 0; c < C; c++) { s[c * 4 + 0] = e.poolBase[c]; s[c * 4 + 1] = e.poolBase[c + 1]; }
+    cudaMemcpyAsync(e.dScalars.p, s, MAX_CTAS * 4 * sizeof(long long), cudaMemcpyHostToDevice, t->stream);
+    a.slot[y] = ManySlot{(const hived_event_t*)e.dEvents.p, (hived_result_t*)e.dResults.p,
+                         e.hasSugg ? (const uint32_t*)e.dSugg.p : nullptr, (int32_t*)e.dPool.p, (long long*)e.dScalars.p,
+                         C > 1 ? (const int32_t*)e.dOwn.p : nullptr, e.stagedN, C, e.nPinnedOrder, e.nBad};
+    devs[y] = &e.dev;
+  }
+  cudaEventRecord(t->start, t->stream);
+  for (int y0 = 0; y0 < k;) {  // one round: the longest prefix of the rest whose (widest C) x (count) fits
+    int y1 = y0 + 1, cmax = a.slot[y0].C;
+    while (y1 < k) {
+      const int c = a.slot[y1].C > cmax ? a.slot[y1].C : cmax;
+      if ((long long)c * (y1 - y0 + 1) > fit) break;
+      cmax = c;
+      y1++;
+    }
+    ManyArgs r;
+    for (int y = y0; y < y1; y++) r.slot[y - y0] = a.slot[y];
+    cudaError_t le = manyLaunch(devs + y0, r, y1 - y0, t->stream);
+    if (le != cudaSuccess) { cudaStreamSynchronize(t->stream); cudaGetLastError(); return fail(std::string("joint launch failed: ") + cudaGetErrorString(le)); }
+    y0 = y1;
+  }
+  cudaEventRecord(t->stop, t->stream);
+  for (int y = 0; y < k; y++)
+    cudaMemcpyAsync(&scal[(size_t)y * MAX_CTAS * 4], es[y]->dScalars.p, MAX_CTAS * 4 * sizeof(long long), cudaMemcpyDeviceToHost, t->stream);
+  cudaError_t ce = cudaStreamSynchronize(t->stream);
+  if (ce != cudaSuccess || (ce = cudaGetLastError()) != cudaSuccess) return fail(std::string("hived_events_many_kernel failed: ") + cudaGetErrorString(ce));
+  float ms = 0.f;
+  cudaEventElapsedTime(&ms, t->start, t->stop);
+  for (int y = 0; y < k; y++) {
+    Engine& e = *es[y];
+    const int C = e.launchCta;
+    const long long* s = &scal[(size_t)y * MAX_CTAS * 4];
+    e.lastKernelMs = ms;
+    e.kernelMsTotal += ms;
+    e.kernelLaunches += C > 1 ? 2 : 1;
+    e.poolEnd.assign(C, 0);
+    for (int c = 0; c < C; c++) e.poolEnd[c] = s[c * 4 + 0];
+    e.poolOff = s[0];
+  }
   return 0;
 }
 

@@ -1,7 +1,8 @@
 // Host side of the library behind include/hived.h: owns the flattened topology, the device memory
 // and the staging buffers; every ABI call becomes an ordered batch of events executed by the device
 // program (hived_core.h).  Included by exactly one translation unit per build:
-//   hived_cuda.cu        -> libhived_cuda.so   (the product: CUDA backend, sm_90a, no host path)
+//   hived_cuda.cu        -> libhived_cuda.so   (the product: CUDA backend, sm_90a, no host path; its second
+//                           translation unit, hived_cuda_many.cu, holds the joint-launch build of the device program)
 //   tests/emu/hived_emu.cpp -> test-only 1-thread emulation of the same device program (HIVED_EMU)
 // The backend supplies bk_* (memory) and launchProgram().
 #pragma once
@@ -15,6 +16,7 @@
 
 #include "../../include/hived.h"
 #include "../../include/hived_hash.h"
+#include "../../include/hived_multictx.h"
 #include "../../include/hived_multigpu.h"
 #include "hived_topo.hpp"
 #define HIVED_TOPO_CONSTS
@@ -43,6 +45,10 @@ int bk_canonicalise(Engine& e, int n, long long* total);
 // copies and kernel queued on the context's stream, ONE synchronisation.  Returns -1 when it does not apply.
 int bk_run_small(Engine& e, const hived_event_t* events, int n, const uint32_t* suggPool, int64_t suggWords, const int32_t* aux,
                  int64_t auxWords, hived_result_t* res, int32_t* pool, int64_t poolCap);
+// runs the staged batches of k contexts of one device together (include/hived_multictx.h) as launchProgram runs one;
+// 0 or HIVED_ERR_PLATFORM (then every listed context's err says why).  A backend that defines HIVED_BK_LAUNCH_MANY
+// before including this header supplies it; the others get the one below, which runs the contexts one after another.
+int bk_launch_many(Engine* const* es, int k);
 void bk_flush_l2();
 
 struct Buf {
@@ -369,6 +375,15 @@ struct Engine {
       int rc = bk_run_small(*this, events, n, suggPool, suggWords, aux, auxWords, res, pool, poolCap);
       if (rc >= 0) { if (rc == 0) trackHealth(events, n); return rc; }
     }
+    int rc = stageBatch(events, n, suggPool, suggWords, aux, auxWords, poolCap);
+    if (rc) return rc;
+    rc = launchProgram(*this, n, false);
+    if (rc) return rc;
+    return collect(events, n, res, pool, poolCap, nullptr);
+  }
+  // the general path's staging (n > 0): prepare() + the suggested-node and aux words to the device
+  int stageBatch(const hived_event_t* events, int n, const uint32_t* suggPool, int64_t suggWords, const int32_t* aux,
+                 int64_t auxWords, int64_t poolCap) {
     prepare(events, n, poolCap);
     hasSugg = suggPool != nullptr && suggWords > 0;
     if (hasSugg) { dSugg.ensure((size_t)suggWords * 4); bk_h2d(dSugg.p, suggPool, (size_t)suggWords * 4); }
@@ -377,10 +392,28 @@ struct Engine {
     poolOff = 0;
     canonicalDone = false;
     if (buffersFailed()) { err = "out of device memory while staging the batch"; return HIVED_ERR_CAPACITY; }
-    int rc = launchProgram(*this, n, false);
-    if (rc) return rc;
+    return 0;
+  }
+  // after the launch of a staged batch: the host mirror of the node health, then results + pool to the caller
+  int collect(const hived_event_t* events, int n, hived_result_t* res, int32_t* pool, int64_t poolCap, int64_t* used) {
     trackHealth(events, n);
-    return fetch(res, pool, poolCap, nullptr);
+    return fetch(res, pool, poolCap, used);
+  }
+  // hived_process_events' verdict on a batch that ran: the running result hash, HIVED_ERR_CAPACITY when an event ran out
+  // of room, and the error text of the first per-event platform error
+  int batchDone(const hived_event_t* events, int n, const hived_result_t* res, const int32_t* pool) {
+    bool noted = false;
+    for (int32_t i = 0; i < n; i++) {
+      if (hashing && events[i].type == HIVED_EV_SCHEDULE) hash = hived_hash_result(hash, &res[i], pool);
+      if (res[i].error == HIVED_ERR_CAPACITY) { err = "capacity exceeded (result pool or hived_options_t)"; return HIVED_ERR_CAPACITY; }
+      if (res[i].error >= 100 && !noted) {  // per-event platform errors stay in the results; the text names the first
+        char buf[128];
+        snprintf(buf, sizeof buf, "event %d failed with platform error %d (see hived_result_t.error of every event)", (int)i, (int)res[i].error);
+        err = buf;
+        noted = true;
+      }
+    }
+    return 0;
   }
   static constexpr int SMALL_BATCH = 8;
   // what prepare() decides per event, for bk_run_small (no device traffic)
@@ -411,6 +444,10 @@ struct Engine {
     return prepare(events, n, poolCap);
   }
   int runStaged() {
+    rearmStaged();
+    return launchProgram(*this, stagedN, false);
+  }
+  void rearmStaged() {
     bk_use_device(deviceOrdinal);
     poolOff = 0;
     canonicalDone = false;
@@ -420,7 +457,6 @@ struct Engine {
       for (int c = 0; c < launchCta; c++) if (ownOff[c + 1] > ownOff[c]) prog[c] = own[ownOff[c]];
       bk_h2d(dev.progress, prog.data(), MAX_CTAS * 4);
     }
-    return launchProgram(*this, stagedN, false);
   }
 
   // ---- multi-GPU partition of one calm batch (include/hived_multigpu.h) --------------------------------------
@@ -632,6 +668,14 @@ struct Engine {
   uint64_t savedHash = HIVED_FNV_OFFSET;
 };
 
+#ifndef HIVED_BK_LAUNCH_MANY
+int bk_launch_many(Engine* const* es, int k) {
+  for (int y = 0; y < k; y++)
+    if (int rc = launchProgram(*es[y], es[y]->stagedN, false)) return rc;
+  return 0;
+}
+#endif
+
 }  // namespace hived
 
 // ================================================================================================
@@ -759,15 +803,50 @@ int hived_process_events(hived_ctx* ctx, const hived_event_t* events, int32_t n,
   hived::Engine& e = ctx->e;
   int rc = e.runBatch(events, n, suggested_pool, suggested_words, nullptr, 0, res, pool, pool_cap);
   if (rc) return rc;
-  bool noted = false;
-  for (int32_t i = 0; i < n; i++) {
-    if (e.hashing && events[i].type == HIVED_EV_SCHEDULE) e.hash = hived_hash_result(e.hash, &res[i], pool);
-    if (res[i].error == HIVED_ERR_CAPACITY) { e.err = "capacity exceeded (result pool or hived_options_t)"; return HIVED_ERR_CAPACITY; }
-    if (res[i].error >= 100 && !noted) {  // per-event platform errors stay in the results; the text names the first
-      char buf[128];
-      snprintf(buf, sizeof buf, "event %d failed with platform error %d (see hived_result_t.error of every event)", (int)i, (int)res[i].error);
-      e.err = buf;
-      noted = true;
+  return e.batchDone(events, n, res, pool);
+}
+
+// ---- include/hived_multictx.h
+// A list the joint launch takes: 1..HIVED_MANY_MAX distinct contexts of one device, none staged for a partition.
+static bool manyListOk(hived_ctx* const* ctxs, int32_t k) {
+  if (k < 1 || k > HIVED_MANY_MAX) return false;
+  for (int32_t i = 0; i < k; i++) {
+    if (!ctxs[i] || !ctxs[i]->e.mgCursor.empty() || ctxs[i]->e.deviceOrdinal != ctxs[0]->e.deviceOrdinal) return false;
+    for (int32_t j = 0; j < i; j++) if (ctxs[j] == ctxs[i]) return false;
+  }
+  return true;
+}
+
+int hived_process_events_many(hived_batch_t* b, int32_t k) {
+  if (k < 1 || k > HIVED_MANY_MAX) return HIVED_ERR_BAD_SPEC;
+  hived_ctx* ctxs[HIVED_MANY_MAX];
+  for (int32_t i = 0; i < k; i++) ctxs[i] = b[i].ctx;
+  if (!manyListOk(ctxs, k)) return HIVED_ERR_BAD_SPEC;
+  // every batch is staged as hived_process_events stages a large one (small batches too: they join the launch); an
+  // empty batch runs nothing, as there
+  hived::Engine* run[HIVED_MANY_MAX];
+  int nRun = 0;
+  for (int32_t i = 0; i < k; i++) {
+    hived::Engine& e = b[i].ctx->e;
+    b[i].rc = 0;
+    b[i].pool_used = 0;
+    if (b[i].n <= 0) continue;
+    hived::bk_use_device(e.deviceOrdinal);
+    b[i].rc = e.stageBatch(b[i].events, b[i].n, b[i].suggested_pool, b[i].suggested_words, nullptr, 0, b[i].pool_cap);
+    if (b[i].rc == 0) run[nRun++] = &e;
+  }
+  if (nRun > 0 && hived::bk_launch_many(run, nRun) != 0) {
+    for (int32_t i = 0; i < k; i++) b[i].rc = HIVED_ERR_PLATFORM;
+    return HIVED_ERR_PLATFORM;
+  }
+  for (int32_t i = 0; i < k; i++) {
+    if (b[i].n <= 0 || b[i].rc != 0) continue;
+    hived::Engine& e = b[i].ctx->e;
+    int64_t used = 0;
+    b[i].rc = e.collect(b[i].events, b[i].n, b[i].res, b[i].pool, b[i].pool_cap, &used);
+    if (b[i].rc == 0) {
+      b[i].pool_used = used;
+      b[i].rc = e.batchDone(b[i].events, b[i].n, b[i].res, b[i].pool);
     }
   }
   return 0;
@@ -940,6 +1019,12 @@ int hived_bench_save_state(hived_ctx* ctx) { ctx->e.saveState(); return 0; }
 int hived_bench_restore_state(hived_ctx* ctx) { return ctx->e.restoreState(); }
 int hived_bench_stage_events(hived_ctx* ctx, const hived_event_t* events, int32_t n, int64_t pool_cap) { return ctx->e.stage(events, n, pool_cap); }
 int hived_bench_run_staged(hived_ctx* ctx) { return ctx->e.runStaged(); }
+int hived_bench_run_staged_many(hived_ctx* const* ctxs, int32_t k) {
+  if (!manyListOk(ctxs, k)) return HIVED_ERR_BAD_SPEC;
+  hived::Engine* run[HIVED_MANY_MAX];
+  for (int32_t i = 0; i < k; i++) { ctxs[i]->e.rearmStaged(); run[i] = &ctxs[i]->e; }
+  return hived::bk_launch_many(run, k);
+}
 int hived_bench_fetch_results(hived_ctx* ctx, hived_result_t* res, int32_t* pool, int64_t pool_cap, int64_t* pool_used) {
   hived::Engine& e = ctx->e;
   return e.fetch(res, pool, pool_cap, pool_used);

@@ -636,6 +636,36 @@ class BatchContext:
             self.ctx = None
 
 
+def process_many(batch_contexts: List[BatchContext], events_list: List[np.ndarray], pool_words_list: List[int],
+                 sugg_pools: List[np.ndarray] = None):
+    """The batches of several contexts of one library and device in one call (hived_process_events_many,
+    include/hived_multictx.h).  Returns [(rc, results, pool)] in list order; each rc is what BatchContext.process's
+    hived_process_events would have returned.  Raises if the call itself fails (a refused list, a failed launch)."""
+    k = len(batch_contexts)
+    lib = _cabi.bind_many(batch_contexts[0].lib)
+    if sugg_pools is None:
+        sugg_pools = [None] * k
+    arr = (_cabi.Batch * max(k, 1))()
+    keep = []
+    for i, (bc, ev, words, sp) in enumerate(zip(batch_contexts, events_list, pool_words_list, sugg_pools)):
+        ev = np.ascontiguousarray(ev)
+        res = np.zeros(len(ev), dtype=RESULT_DT)
+        pool = np.zeros(max(int(words), 1), dtype=np.int32)
+        b = arr[i]
+        b.ctx, b.n, b.pool_cap = bc.ctx, len(ev), int(words)
+        b.events = ev.ctypes.data_as(C.POINTER(_cabi.Event))
+        b.res = res.ctypes.data_as(C.POINTER(_cabi.Result))
+        b.pool = pool.ctypes.data_as(C.POINTER(C.c_int32))
+        if sp is not None and len(sp):
+            sp = np.ascontiguousarray(sp, dtype=np.uint32)
+            b.suggested_pool, b.suggested_words = sp.ctypes.data_as(C.POINTER(C.c_uint32)), len(sp)
+        keep.append((ev, res, pool, sp))
+    rc = lib.hived_process_events_many(arr, k)
+    if rc != 0:
+        raise RuntimeError("hived_process_events_many failed (%d)" % rc)
+    return [(arr[i].rc, keep[i][1], keep[i][2]) for i in range(k)]
+
+
 def pool_words_for(trace: Dict[str, Any]) -> int:
     """Upper bound of result-pool words: every SCHEDULE event may emit the whole gang placement."""
     ev = trace["events"]

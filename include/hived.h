@@ -11,7 +11,8 @@
  * Threads: a context is used by one thread at a time (the reference serialises every SchedulerAlgorithm call behind
  *   its algorithmLock, hived_algorithm.go:104, and the shims keep that lock).  Different contexts may be driven by
  *   different threads; contexts that live on the same GPU take turns there (the device-side view of a context's state
- *   sits in the device's constant bank, one context at a time: a process-wide lock inside the library).
+ *   sits in the device's constant bank, one context at a time: a process-wide lock inside the library).  To run the
+ *   batches of several contexts on one GPU at the same time, hand them to one call: hived_multictx.h.
  * Conventions
  *   - plain C, ints and pointers only, no callbacks, nothing retained after a call returns;
  *   - every buffer is caller-owned; results are written into caller-provided arrays;

@@ -11,6 +11,9 @@ int hived_bench_save_state(hived_ctx*);     /* device-to-device copy of every mu
 int hived_bench_restore_state(hived_ctx*);
 int hived_bench_stage_events(hived_ctx*, const hived_event_t* events, int32_t n, int64_t pool_cap); /* H2D once */
 int hived_bench_run_staged(hived_ctx*);     /* one kernel launch over the staged batch; nothing crosses PCIe */
+/* the staged batches of k contexts in one joint launch (hived_multictx.h); each context's hived_bench_last_kernel_ms
+   then reports the joint launch.  HIVED_ERR_BAD_SPEC for a list hived_process_events_many refuses */
+int hived_bench_run_staged_many(hived_ctx* const* ctxs, int32_t k);
 int hived_bench_fetch_results(hived_ctx*, hived_result_t* res, int32_t* pool, int64_t pool_cap, int64_t* pool_used);
 int hived_bench_flush_l2(hived_ctx*);       /* overwrite a buffer larger than L2 */
 /* out[0..15): SM cycles of the leader warps in {view pass, leaf search, v->p mapping, result emission, commit, delete,
