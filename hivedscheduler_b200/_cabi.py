@@ -16,6 +16,8 @@ GROUP_NONE, GROUP_ALLOCATED, GROUP_PREEMPTING, GROUP_BEING_PREEMPTED = 0, 1, 2, 
 WAIT_INSUFFICIENT, WAIT_BAD_NODE, WAIT_NON_SUGGESTED_NODE, WAIT_MAPPING, WAIT_NO_SCHEDULER = 1, 2, 3, 4, 5
 WAIT_SCOPE_VC, WAIT_SCOPE_PHYSICAL = 16, 32
 ERR_PLATFORM = 100
+OPT_NO_RESULT_HASH, OPT_CONCURRENT = 1, 2  # hived_options_t.flags
+HIVED_CONCURRENT_MAX = 16                  # HIVED_OPT_CONCURRENT contexts per device
 
 _M = C.c_int32 * HIVED_MAX_MEMBERS
 

@@ -97,8 +97,11 @@ __shared__ Sm g_hived_sm;  // one per CTA (both kernels of hived_cuda.cu use it)
 // context's Dev is loaded per device at a time; launchProgram / the per-call path reload it when the owner changes
 // (hived_cuda.cu: ensureDevLoaded).
 #ifdef HIVED_MANY_BUILD
-// Joint launches (include/hived_multictx.h): one Dev per listed context, CTA (x, y) is CTA x of context y.
-__constant__ Dev g_hived_devs[HIVED_MANY_MAX];
+// Joint launches (include/hived_multictx.h): one Dev per listed context, CTA (x, y) is CTA x of context y, in slots
+// [0, HIVED_MANY_MAX).  Slots [HIVED_MANY_MAX, HIVED_MANY_MAX + HIVED_CONCURRENT_MAX) belong to the concurrent contexts
+// of the device (HIVED_OPT_CONCURRENT), one each for the context's whole life, read by its resident per-call kernel.
+__constant__ Dev g_hived_devs[HIVED_MANY_MAX + HIVED_CONCURRENT_MAX];
+static_assert((HIVED_MANY_MAX + HIVED_CONCURRENT_MAX) * sizeof(Dev) <= 64 * 1024, "the Dev slots must fit the 64 KB constant bank");
 #else
 __constant__ Dev g_hived_dev;
 #endif

@@ -13,6 +13,7 @@
 #include <mutex>
 
 #define HIVED_BK_LAUNCH_MANY 1  // the joint launch below
+#define HIVED_BK_CONCURRENT 1   // concurrent contexts' own resident kernels below
 #include "hived_engine.hpp"
 #include "hived_many.h"
 
@@ -135,62 +136,184 @@ int bk_init(int& device, std::string& err) {
   return 0;
 }
 
-struct CudaTimers {
-  cudaEvent_t start = nullptr, stop = nullptr;
+// A resident per-call kernel (bk_run_small): a non-blocking stream of its own, one request slot in mapped host memory
+// and the device staging of the events it runs.
+struct ServeChan {
   cudaStream_t stream = nullptr;
-  // resident per-call kernel (bk_run_small): a non-blocking stream of its own, one request slot in mapped host memory
-  cudaStream_t serveStream = nullptr;
+  cudaStream_t copyStream = nullptr;     // concurrent kernels: the pool words beyond the slot's window
   volatile int32_t* slotHost = nullptr;  // cudaHostAlloc(mapped)
   int32_t* slotDev = nullptr;
   hived_result_t* stageRes = nullptr;
   uint32_t* dSugg = nullptr;
   int32_t* dAux = nullptr;
-  int32_t* servePool = nullptr;
-  long long servePoolCap = 0;
+  int32_t* pool = nullptr;
+  long long poolCap = 0;
   int seq = 0;
+  int conc = -1;         // -1: hived_serve_kernel on g_hived_dev; else the concurrent slot its hived_serve_many_kernel reads
   bool alive = false;    // a serve kernel was launched and has not been seen to exit
-  bool disabled = false; // HIVED_NO_RESIDENT=1, or setting it up failed: one launch per call
   long long served = 0, launches = 0;
 };
+
+struct CudaTimers {
+  cudaEvent_t start = nullptr, stop = nullptr;
+  cudaStream_t stream = nullptr;
+  ServeChan serve;       // the resident kernel of the turn-taking path (g_hived_dev)
+  bool disabled = false; // HIVED_NO_RESIDENT=1, or setting it up failed: one launch per call
+  ServeChan* conc = nullptr;  // a concurrent context's own resident kernel (bk_open_concurrent); nullptr otherwise
+};
+
+static bool noResident() {
+  const char* off = getenv("HIVED_NO_RESIDENT");
+  return off && *off && *off != '0';
+}
+
+// Stop a resident kernel (if any) and wait until it has left.
+static void serveStop(ServeChan& c) {
+  if (!c.alive) return;
+  volatile int32_t* s = c.slotHost;
+  if (!s[SERVE_DONE_OFF + 4]) {
+    s[1] = 0;  // n = 0: STOP
+    __sync_synchronize();
+    s[0] = ++c.seq;
+  }
+  cudaStreamSynchronize(c.stream);
+  c.alive = false;
+}
 
 // ---- whose Dev is in the constant bank (g_hived_dev, hived_core.h) of each device ---------------------------------
 // One context per device at a time.  Every section that launches a kernel or talks to a resident one holds g_devMu
 // (contexts of one process take turns on the GPU; a context by itself is single-threaded per the ABI), makes sure its
 // own Dev is the one loaded, and leaves nothing of its own running except the resident per-call kernel — which the
-// next owner stops (bk_quiesce) before it overwrites the constant bank.
+// next owner stops before it overwrites the constant bank.  A concurrent context's own resident kernel
+// (HIVED_OPT_CONCURRENT, below) reads another constant slot and is never stopped from here: only its own caller stops
+// it (bk_quiesce), since another thread's stop would race with that caller's call in flight.
 static std::recursive_mutex g_devMu;
 static Engine* g_devOwner[64] = {nullptr};
 
-void bk_quiesce(Engine& e);
 static int ensureDevLoaded(Engine& e) {  // g_devMu held, the context's device current
   const int dv = e.deviceOrdinal >= 0 && e.deviceOrdinal < 64 ? e.deviceOrdinal : 0;
   if (g_devOwner[dv] == &e) return 0;
-  if (g_devOwner[dv]) bk_quiesce(*g_devOwner[dv]);
+  if (g_devOwner[dv]) serveStop(((CudaTimers*)g_devOwner[dv]->stream)->serve);
   g_devOwner[dv] = nullptr;
   cudaError_t ce = cudaMemcpyToSymbol(g_hived_dev, &e.dev, sizeof(Dev));  // synchronous: nothing of ours is running
   if (ce != cudaSuccess) { e.err = std::string("cudaMemcpyToSymbol(g_hived_dev): ") + cudaGetErrorString(ce); return HIVED_ERR_PLATFORM; }
   g_devOwner[dv] = &e;
   return 0;
 }
+static void concClose(Engine& e);
 void bk_forget(Engine& e) {  // the context is going away
-  std::lock_guard<std::recursive_mutex> lk(g_devMu);
-  for (auto& o : g_devOwner) if (o == &e) o = nullptr;
+  {
+    std::lock_guard<std::recursive_mutex> lk(g_devMu);
+    for (auto& o : g_devOwner) if (o == &e) o = nullptr;
+  }
+  concClose(e);
 }
 
-// Stop the resident kernel (if any) and wait until it has left: before anything else launches on or writes to the
-// scheduler state.  Called with the context's device current.
+// Stop the context's resident kernels (if any) and wait until they have left: before anything else launches on or
+// writes to the scheduler state.  Called by the context's own caller, with the context's device current.
 void bk_quiesce(Engine& e) {
   std::lock_guard<std::recursive_mutex> lk(g_devMu);
   CudaTimers* t = (CudaTimers*)e.stream;
-  if (!t || !t->alive) return;
-  volatile int32_t* s = t->slotHost;
-  if (!s[SERVE_DONE_OFF + 4]) {
-    s[1] = 0;  // n = 0: STOP
-    __sync_synchronize();
-    s[0] = ++t->seq;
+  if (!t) return;
+  serveStop(t->serve);
+  if (t->conc) serveStop(*t->conc);
+}
+
+// ---- concurrent contexts (HIVED_OPT_CONCURRENT) --------------------------------------------------------------------
+// Each holds one of the device's HIVED_CONCURRENT_MAX slots from hived_create to hived_destroy: its Dev sits in constant
+// slot HIVED_MANY_MAX + s of the joint build (hived_cuda_many.cu), copied once, and its per-call path runs on a resident
+// kernel of its own (hived_serve_many_kernel) through a request slot of its own, without g_devMu.
+// Invariant: a slot's Dev is written only while no kernel that reads that slot runs (the slot is free: the previous
+// holder's kernel was stopped before it gave the slot back), and the kernel that reads it is launched after the write
+// has completed.  Writes to other slots — another context's creation, a joint launch's slots 0..k-1 — may happen while
+// resident kernels run.
+static std::mutex g_concMu;
+static Engine* g_concSlot[64][HIVED_CONCURRENT_MAX] = {};
+
+// Resident CTAs of concurrent kernels that may be live on the device at any moment (one per slot taken, whether its
+// kernel runs now or not: another thread may launch it at any time).
+static int concInUse(int dv) {
+  std::lock_guard<std::mutex> lk(g_concMu);
+  int n = 0;
+  for (Engine* o : g_concSlot[dv]) n += o != nullptr;
+  return n;
+}
+
+// Device staging of a resident kernel's channel; false if something could not be allocated.
+static bool serveAlloc(const Engine& e, ServeChan& c) {
+  void* h = nullptr;
+  if (cudaStreamCreateWithFlags(&c.stream, cudaStreamNonBlocking) != cudaSuccess ||
+      cudaHostAlloc(&h, (size_t)SERVE_SLOT_WORDS * 4, cudaHostAllocMapped) != cudaSuccess) return false;
+  memset(h, 0, (size_t)SERVE_SLOT_WORDS * 4);
+  c.slotHost = (volatile int32_t*)h;
+  void* d = nullptr;
+  if (cudaHostGetDevicePointer(&d, h, 0) != cudaSuccess) return false;
+  c.slotDev = (int32_t*)d;
+  c.poolCap = 3ll * e.dev.S.LS + 2 * 4096 + 64 > SERVE_POOL_WINDOW ? 3ll * e.dev.S.LS + 2 * 4096 + 64 : SERVE_POOL_WINDOW;
+  c.poolCap *= SERVE_MAX_EVENTS;
+  return cudaMalloc((void**)&c.stageRes, sizeof(hived_result_t) * SERVE_MAX_EVENTS) == cudaSuccess &&
+         cudaMalloc((void**)&c.dSugg, (size_t)SERVE_SUGG_MAX * 4) == cudaSuccess &&
+         cudaMalloc((void**)&c.dAux, (size_t)SERVE_AUX_MAX * 4) == cudaSuccess &&
+         cudaMalloc((void**)&c.pool, (size_t)c.poolCap * 4) == cudaSuccess;
+}
+
+static void serveFree(ServeChan& c) {  // the kernel has left
+  cudaFree(c.stageRes); cudaFree(c.dSugg); cudaFree(c.dAux); cudaFree(c.pool);
+  if (c.slotHost) cudaFreeHost((void*)c.slotHost);
+  if (c.copyStream) cudaStreamDestroy(c.copyStream);
+  if (c.stream) cudaStreamDestroy(c.stream);
+}
+
+// The largest cooperative grid of one context (launchProgram: one CTA per VC, at most 16).  A device keeps this many
+// co-resident CTAs free of concurrent kernels, so that such a grid always fits beside them.
+constexpr int COOP_CTAS_MAX = 16;
+
+int bk_open_concurrent(Engine& e) {  // the end of hived_create: the device is current
+  const int dv = e.deviceOrdinal >= 0 && e.deviceOrdinal < 64 ? e.deviceOrdinal : 0;
+  const int fit = manyCoResident(e.deviceOrdinal);
+  const int cap = fit - COOP_CTAS_MAX < HIVED_CONCURRENT_MAX ? fit - COOP_CTAS_MAX : HIVED_CONCURRENT_MAX;
+  int slot = -1;
+  {
+    std::lock_guard<std::mutex> lk(g_concMu);
+    int used = 0;
+    for (int s = 0; s < HIVED_CONCURRENT_MAX; s++) {
+      if (g_concSlot[dv][s]) used++;
+      else if (slot < 0) slot = s;
+    }
+    if (used >= cap) {
+      char buf[200];
+      snprintf(buf, sizeof buf, "HIVED_OPT_CONCURRENT: all %d concurrent-context slots of device %d are taken "
+               "(HIVED_CONCURRENT_MAX per device)", cap > 0 ? cap : 0, dv);
+      e.err = buf;
+      return HIVED_ERR_CAPACITY;
+    }
+    g_concSlot[dv][slot] = &e;
   }
-  cudaStreamSynchronize(t->serveStream);
-  t->alive = false;
+  if (noResident()) return 0;  // the slot is held, but every call takes turns
+  CudaTimers* t = (CudaTimers*)e.stream;
+  ServeChan* c = new ServeChan();
+  c->conc = slot;
+  t->conc = c;
+  if (!serveAlloc(e, *c) || cudaStreamCreateWithFlags(&c->copyStream, cudaStreamNonBlocking) != cudaSuccess) {
+    e.err = "out of device or pinned host memory for the concurrent context's resident kernel";
+    return HIVED_ERR_CAPACITY;
+  }
+  cudaError_t ce = concLoadDev(e.dev, slot, c->stream);
+  if (ce == cudaSuccess) ce = cudaStreamSynchronize(c->stream);
+  if (ce != cudaSuccess) { e.err = std::string("copying the Dev into its concurrent slot: ") + cudaGetErrorString(ce); return HIVED_ERR_PLATFORM; }
+  return 0;
+}
+
+static void concClose(Engine& e) {  // bk_quiesce has stopped the kernel
+  CudaTimers* t = (CudaTimers*)e.stream;
+  if (t && t->conc) {
+    serveFree(*t->conc);
+    delete t->conc;
+    t->conc = nullptr;
+  }
+  std::lock_guard<std::mutex> lk(g_concMu);
+  for (auto& dev : g_concSlot)
+    for (Engine*& o : dev) if (o == &e) o = nullptr;
 }
 
 static_assert(NT / 32 <= MAX_WARPS, "the shared counters are sized for MAX_WARPS warps per CTA");
@@ -287,14 +410,15 @@ int bk_launch_many(Engine* const* es, int k) {
   Engine& e0 = *es[0];
   const int dv = e0.deviceOrdinal >= 0 && e0.deviceOrdinal < 64 ? e0.deviceOrdinal : 0;
   for (int y = 0; y < k; y++) bk_quiesce(*es[y]);
-  if (g_devOwner[dv]) bk_quiesce(*g_devOwner[dv]);
+  if (g_devOwner[dv]) serveStop(((CudaTimers*)g_devOwner[dv]->stream)->serve);
   auto fail = [&](const std::string& why) {
     for (int y = 0; y < k; y++) es[y]->err = why;
     return HIVED_ERR_PLATFORM;
   };
   std::string err;
   if (takeCopyError(err)) return fail(err);  // a staging copy of one of the batches failed
-  const int fit = manyCoResident(e0.deviceOrdinal);
+  // the concurrent contexts' resident CTAs may come and go during the launch (other threads): leave them one SM each
+  const int fit = manyCoResident(e0.deviceOrdinal) - concInUse(dv);
   if (fit <= 0) return fail("joint launch: cannot query the co-resident CTA limit");
   CudaTimers* t = (CudaTimers*)e0.stream;
   std::vector<long long> scal((size_t)k * MAX_CTAS * 4, 0);
@@ -364,44 +488,35 @@ static constexpr int64_t SMALL_POOL_WINDOW = 16384;  // words copied back with t
 // stream synchronisation per call.  The kernel leaves after ~2 ms without a request and is relaunched on demand.
 static bool serveSetup(Engine& e, CudaTimers* t) {
   if (t->disabled) return false;
-  if (t->slotHost) return true;
-  const char* off = getenv("HIVED_NO_RESIDENT");
-  if (off && *off && *off != '0') { t->disabled = true; return false; }
-  void* h = nullptr;
-  if (cudaStreamCreateWithFlags(&t->serveStream, cudaStreamNonBlocking) != cudaSuccess ||
-      cudaHostAlloc(&h, (size_t)SERVE_SLOT_WORDS * 4, cudaHostAllocMapped) != cudaSuccess) { t->disabled = true; return false; }
-  memset(h, 0, (size_t)SERVE_SLOT_WORDS * 4);
-  t->slotHost = (volatile int32_t*)h;
-  void* d = nullptr;
-  if (cudaHostGetDevicePointer(&d, h, 0) != cudaSuccess) { t->disabled = true; return false; }
-  t->slotDev = (int32_t*)d;
-  t->servePoolCap = 3ll * e.dev.S.LS + 2 * 4096 + 64 > SERVE_POOL_WINDOW ? 3ll * e.dev.S.LS + 2 * 4096 + 64 : SERVE_POOL_WINDOW;
-  t->servePoolCap *= SERVE_MAX_EVENTS;
-  if (cudaMalloc((void**)&t->stageRes, sizeof(hived_result_t) * SERVE_MAX_EVENTS) != cudaSuccess ||
-      cudaMalloc((void**)&t->dSugg, (size_t)SERVE_SUGG_MAX * 4) != cudaSuccess || cudaMalloc((void**)&t->dAux, (size_t)SERVE_AUX_MAX * 4) != cudaSuccess ||
-      cudaMalloc((void**)&t->servePool, (size_t)t->servePoolCap * 4) != cudaSuccess) { t->disabled = true; return false; }
+  if (t->serve.slotHost) return true;
+  if (noResident() || !serveAlloc(e, t->serve)) { t->disabled = true; return false; }
   cudaFuncSetAttribute(hived_serve_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 10);
   return true;
 }
 
-static int serveCall(Engine& e, CudaTimers* t, const hived_event_t* events, int n, const uint32_t* suggPool, int64_t suggWords,
+// what the resident kernel's request slot holds
+static bool serveTakes(int n, const uint32_t* suggPool, int64_t suggWords, const int32_t* aux, int64_t auxWords) {
+  const bool hasSugg = suggPool != nullptr && suggWords > 0, hasAux = aux != nullptr && auxWords > 0;
+  return n <= SERVE_MAX_EVENTS && !(hasSugg && suggWords > SERVE_SUGG_MAX) && !(hasAux && auxWords > SERVE_AUX_MAX);
+}
+
+// One call through a resident kernel's channel (serveTakes holds, the channel is set up).
+static int serveCall(Engine& e, ServeChan& c, const hived_event_t* events, int n, const uint32_t* suggPool, int64_t suggWords,
                      const int32_t* aux, int64_t auxWords, hived_result_t* res, int32_t* pool, int64_t poolCap) {
   const bool hasSugg = suggPool != nullptr && suggWords > 0, hasAux = aux != nullptr && auxWords > 0;
-  if (n > SERVE_MAX_EVENTS || (hasSugg && suggWords > SERVE_SUGG_MAX) || (hasAux && auxWords > SERVE_AUX_MAX)) return -2;
-  if (!serveSetup(e, t)) return -2;
-  const long long cap = poolCap < t->servePoolCap ? poolCap : t->servePoolCap;
+  const long long cap = poolCap < c.poolCap ? poolCap : c.poolCap;
   e.notePriorities(events, n);
   e.launchCta = 1;
   e.hasSugg = hasSugg; e.hasAux = hasAux;
   e.poolCapWords = poolCap; e.stagedN = n; e.stagedEvents = events; e.canonicalDone = false;
-  volatile int32_t* s = t->slotHost;
+  volatile int32_t* s = c.slotHost;
   int32_t* pay = (int32_t*)(s + SERVE_EV_OFF);
   memcpy(pay, events, (size_t)n * sizeof(hived_event_t));
   int32_t* hs = pay + SERVE_MAX_EVENTS * (int)(sizeof(hived_event_t) / 4);
   if (hasSugg) memcpy(hs, suggPool, (size_t)suggWords * 4);
   if (hasAux) memcpy(hs + (hasSugg ? suggWords : 0), aux, (size_t)auxWords * 4);
   s[1] = n; s[2] = hasSugg ? (int32_t)suggWords : 0; s[3] = hasAux ? (int32_t)auxWords : 0; s[4] = (int32_t)cap;
-  const int seq = ++t->seq;
+  const int seq = ++c.seq;
   __sync_synchronize();
   s[0] = seq;
   auto launch = [&]() {
@@ -409,27 +524,33 @@ static int serveCall(Engine& e, CudaTimers* t, const hived_event_t* events, int 
     __sync_synchronize();
     // 1500 polls over PCIe: the kernel leaves after 1.5-2 ms without a request on an H100
     // (profiles/micro/resident_idle_timeout.py)
-    hived_serve_kernel<<<1, NT, 0, t->serveStream>>>(t->slotDev, seq - 1, 1500, t->stageRes, t->dSugg, t->dAux, e.nPinnedOrder,
-                                                      e.nBad, t->servePool);
-    t->alive = true;
-    t->launches++;
+    cudaError_t le = cudaSuccess;
+    if (c.conc < 0)
+      hived_serve_kernel<<<1, NT, 0, c.stream>>>(c.slotDev, seq - 1, 1500, c.stageRes, c.dSugg, c.dAux, e.nPinnedOrder, e.nBad,
+                                                 c.pool);
+    else
+      le = concServeLaunch(c.conc, c.slotDev, seq - 1, 1500, c.stageRes, c.dSugg, c.dAux, e.nPinnedOrder, e.nBad, c.pool, c.stream);
+    if (le != cudaSuccess) { e.err = std::string("launching hived_serve_many_kernel failed: ") + cudaGetErrorString(le); return false; }
+    c.alive = true;
+    c.launches++;
     e.kernelLaunches++;
+    return true;
   };
-  if (!t->alive) launch();
+  if (!c.alive && !launch()) return HIVED_ERR_PLATFORM;
   // wait for `done`; a kernel that left just before the request arrived is replaced
   long long spins = 0;
   while (s[SERVE_DONE_OFF] != seq) {
     if (s[SERVE_DONE_OFF + 4] && s[SERVE_DONE_OFF] != seq) {
-      cudaError_t err = cudaStreamSynchronize(t->serveStream);
-      if (err != cudaSuccess) { e.err = std::string("hived_serve_kernel failed: ") + cudaGetErrorString(err); t->alive = false; return HIVED_ERR_PLATFORM; }
+      cudaError_t err = cudaStreamSynchronize(c.stream);
+      if (err != cudaSuccess) { e.err = std::string("hived_serve_kernel failed: ") + cudaGetErrorString(err); c.alive = false; return HIVED_ERR_PLATFORM; }
       if (s[SERVE_DONE_OFF] == seq) break;
-      launch();
+      if (!launch()) { c.alive = false; return HIVED_ERR_PLATFORM; }
     }
     if ((++spins & 0xfffff) == 0) {  // every ~million polls: is the kernel still healthy?
-      cudaError_t err = cudaStreamQuery(t->serveStream);
+      cudaError_t err = cudaStreamQuery(c.stream);
       if (err != cudaSuccess && err != cudaErrorNotReady) {
         e.err = std::string("hived_serve_kernel failed: ") + cudaGetErrorString(err);
-        t->alive = false;
+        c.alive = false;
         return HIVED_ERR_PLATFORM;
       }
     }
@@ -438,7 +559,7 @@ static int serveCall(Engine& e, CudaTimers* t, const hived_event_t* events, int 
 #endif
   }
   __sync_synchronize();
-  t->served++;
+  c.served++;
   const long long used = (long long)(uint32_t)s[SERVE_DONE_OFF + 1] | ((long long)s[SERVE_DONE_OFF + 2] << 32);
   e.poolOff = used;
   e.poolEnd.assign(1, used);
@@ -447,21 +568,33 @@ static int serveCall(Engine& e, CudaTimers* t, const hived_event_t* events, int 
   memcpy(res, (const void*)(s + SERVE_RES_OFF), (size_t)n * sizeof(hived_result_t));
   const long long got = used < SERVE_POOL_WINDOW ? used : SERVE_POOL_WINDOW;
   if (got > 0) memcpy(pool, (const void*)(s + SERVE_RES_OFF + SERVE_MAX_EVENTS * (int)(sizeof(hived_result_t) / 4)), (size_t)got * 4);
-  if (used > SERVE_POOL_WINDOW)
-    cudaMemcpy(pool + SERVE_POOL_WINDOW, t->servePool + SERVE_POOL_WINDOW, (size_t)(used - SERVE_POOL_WINDOW) * 4, cudaMemcpyDeviceToHost);
+  if (used > SERVE_POOL_WINDOW) {
+    int32_t* dst = pool + SERVE_POOL_WINDOW;
+    const int32_t* src = c.pool + SERVE_POOL_WINDOW;
+    const size_t bytes = (size_t)(used - SERVE_POOL_WINDOW) * 4;
+    if (c.conc < 0) {
+      cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost);
+    } else {  // a concurrent context synchronises with nothing but its own copy stream
+      cudaError_t ce = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, c.copyStream);
+      if (ce == cudaSuccess) ce = cudaStreamSynchronize(c.copyStream);
+      if (ce != cudaSuccess) { e.err = std::string("copying the pool words beyond the window: ") + cudaGetErrorString(ce); return HIVED_ERR_PLATFORM; }
+    }
+  }
   return 0;
 }
 
 int bk_run_small(Engine& e, const hived_event_t* events, int n, const uint32_t* suggPool, int64_t suggWords, const int32_t* aux,
                  int64_t auxWords, hived_result_t* res, int32_t* pool, int64_t poolCap) {
   if (!e.stream) return -1;  // the first launch (initialisation) creates the stream
-  std::lock_guard<std::recursive_mutex> lk(g_devMu);
   CudaTimers* t = (CudaTimers*)e.stream;
+  const bool takes = serveTakes(n, suggPool, suggWords, aux, auxWords);
+  // a concurrent context: its own resident kernel and constant slot, no g_devMu, no turn on g_hived_dev
+  if (t->conc && takes) return serveCall(e, *t->conc, events, n, suggPool, suggWords, aux, auxWords, res, pool, poolCap);
+  std::lock_guard<std::recursive_mutex> lk(g_devMu);
+  if (t->conc) serveStop(*t->conc);  // (a call its kernel does not take) the launch below writes the same state
   if (int rc = ensureDevLoaded(e)) return rc;
-  {
-    int rc = serveCall(e, t, events, n, suggPool, suggWords, aux, auxWords, res, pool, poolCap);
-    if (rc != -2) return rc;  // -2: the resident path does not take this call
-  }
+  if (!t->conc && takes && serveSetup(e, t))
+    return serveCall(e, t->serve, events, n, suggPool, suggWords, aux, auxWords, res, pool, poolCap);
   static thread_local SmallStage stage;  // per host thread; the shim serialises calls per context anyway
   const bool hasSugg = suggPool != nullptr && suggWords > 0, hasAux = aux != nullptr && auxWords > 0;
   const int64_t window = poolCap < SMALL_POOL_WINDOW ? poolCap : SMALL_POOL_WINDOW;

@@ -49,6 +49,10 @@ int bk_run_small(Engine& e, const hived_event_t* events, int n, const uint32_t* 
 // 0 or HIVED_ERR_PLATFORM (then every listed context's err says why).  A backend that defines HIVED_BK_LAUNCH_MANY
 // before including this header supplies it; the others get the one below, which runs the contexts one after another.
 int bk_launch_many(Engine* const* es, int k);
+// the end of hived_create for a context with HIVED_OPT_CONCURRENT: the backend gives it a resident per-call kernel of its
+// own (0, or HIVED_ERR_* with err set).  A backend that defines HIVED_BK_CONCURRENT supplies it; the others accept the
+// flag and ignore it.
+int bk_open_concurrent(Engine& e);
 void bk_flush_l2();
 
 struct Buf {
@@ -240,6 +244,7 @@ struct Engine {
     }
     rc = launchProgram(*this, 0, true);
     if (rc) { if (err.empty()) err = "device initialisation failed"; return rc; }
+    if (opt.flags & HIVED_OPT_CONCURRENT) return bk_open_concurrent(*this);
     return 0;
   }
 
@@ -674,6 +679,9 @@ int bk_launch_many(Engine* const* es, int k) {
     if (int rc = launchProgram(*es[y], es[y]->stagedN, false)) return rc;
   return 0;
 }
+#endif
+#ifndef HIVED_BK_CONCURRENT
+int bk_open_concurrent(Engine&) { return 0; }
 #endif
 
 }  // namespace hived

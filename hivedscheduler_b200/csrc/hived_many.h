@@ -30,4 +30,12 @@ int manyCoResident(int device);
 // the joint repair kernel for those contexts.  Everything is queued on `st`; the caller synchronises.
 cudaError_t manyLaunch(const Dev* const* devs, const ManyArgs& a, int k, cudaStream_t st);
 
+// concurrent contexts (HIVED_OPT_CONCURRENT): concurrent slot s (0 <= s < HIVED_CONCURRENT_MAX) is constant slot
+// HIVED_MANY_MAX + s.  concLoadDev queues the copy of the context's Dev into it on `st`; the caller synchronises before
+// the first launch.  concServeLaunch queues the slot's resident per-call kernel (Core::serve, arguments as for
+// hived_serve_kernel) on `st`.
+cudaError_t concLoadDev(const Dev& dev, int s, cudaStream_t st);
+cudaError_t concServeLaunch(int s, volatile int32_t* slot, int seq0, int idleSpins, hived_result_t* stageRes, uint32_t* dSugg,
+                            int32_t* dAux, int nPinnedOrder, int nBad, int32_t* pool, cudaStream_t st);
+
 }  // namespace hived

@@ -579,14 +579,15 @@ def run_c4_compiled(lib, config, n_gangs: int, n_vcs: int, vc_gpus: int, total_g
 # ------------------------------------------------------------------------------------------------
 
 class BatchContext:
-    """A raw ctx of include/hived.h for the batch path (bench.py, parity tests)."""
+    """A raw ctx of include/hived.h for the batch path (bench.py, parity tests).  flags: hived_options_t.flags
+    (_cabi.OPT_*)."""
 
     def __init__(self, lib, config: Dict[str, Any], max_groups: int, max_pods: int, max_group_leaves: int = 64,
-                 max_group_pods: int = 8, device: int = 0):
+                 max_group_pods: int = 8, device: int = 0, flags: int = 0):
         from .config import to_spec_text
         self.lib = lib
         self.opt = _cabi.Options(max_groups=max_groups, max_pods=max_pods, max_group_leaves=max_group_leaves,
-                                 max_group_pods=max_group_pods, device=device)
+                                 max_group_pods=max_group_pods, device=device, flags=flags)
         self.ctx = C.c_void_p()
         rc = lib.hived_create(to_spec_text(config).encode(), C.byref(self.opt), C.byref(self.ctx))
         if rc != 0:

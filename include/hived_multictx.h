@@ -10,6 +10,12 @@
  *
  * Threads: the caller holds every listed context (the single-writer rule of hived.h).  Contexts that are not listed
  * keep taking turns on the device through the ordinary calls.
+ *
+ * Concurrent contexts (HIVED_OPT_CONCURRENT, hived.h) may be listed like any other: the call first stops the resident
+ * per-call kernel of each listed context (the caller holds it, so none of its calls is in flight) and its next per-call
+ * operation starts a new one.  Concurrent contexts that are not listed keep answering their own threads' calls during
+ * the joint call; the launch leaves one SM per concurrent context of the device to them, so a list may need one more
+ * round than it would on an otherwise idle device.
  */
 #ifndef HIVED_MULTICTX_H_
 #define HIVED_MULTICTX_H_
