@@ -33,8 +33,10 @@ namespace hived {
 #ifdef HIVED_MANY_BUILD
 // The second build of the program (hived_cuda_many.cu, joint launches of several contexts) lives in a namespace of its
 // own: the out-of-line members of Core would otherwise have the same names in both builds, and one copy would be
-// dropped at link time.
+// dropped at link time.  So does the third (hived_cuda_conc.cu, concurrent contexts).
 namespace many {
+#elif defined(HIVED_CONC_BUILD)
+namespace conc {
 #endif
 
 #ifndef HIVED_TOPO_CONSTS
@@ -98,10 +100,20 @@ __shared__ Sm g_hived_sm;  // one per CTA (both kernels of hived_cuda.cu use it)
 // (hived_cuda.cu: ensureDevLoaded).
 #ifdef HIVED_MANY_BUILD
 // Joint launches (include/hived_multictx.h): one Dev per listed context, CTA (x, y) is CTA x of context y, in slots
-// [0, HIVED_MANY_MAX).  Slots [HIVED_MANY_MAX, HIVED_MANY_MAX + HIVED_CONCURRENT_MAX) belong to the concurrent contexts
-// of the device (HIVED_OPT_CONCURRENT), one each for the context's whole life, read by its resident per-call kernel.
-__constant__ Dev g_hived_devs[HIVED_MANY_MAX + HIVED_CONCURRENT_MAX];
-static_assert((HIVED_MANY_MAX + HIVED_CONCURRENT_MAX) * sizeof(Dev) <= 64 * 1024, "the Dev slots must fit the 64 KB constant bank");
+// [0, HIVED_MANY_MAX).
+__constant__ Dev g_hived_devs[HIVED_MANY_MAX];
+#elif defined(HIVED_CONC_BUILD)
+// Concurrent contexts (HIVED_OPT_CONCURRENT): slot s belongs to the context in concurrent slot s of the device for its
+// whole life, read by its resident per-call kernel and its batches.  A launch names its slot by its dynamic
+// shared-memory byte count (hv_slot_base); the kernels declare no dynamic shared memory, so the bytes are only a tag.
+// The value is uniform over the launch: one uniform constant load, kept in a uniform register.
+__constant__ Dev g_hived_devs[HIVED_CONCURRENT_MAX];
+static_assert(HIVED_CONCURRENT_MAX * sizeof(Dev) <= 64 * 1024, "the Dev slots must fit the 64 KB constant bank");
+__device__ __forceinline__ unsigned hv_slot_base() {
+  unsigned r;
+  asm("mov.u32 %0, %%dynamic_smem_size;" : "=r"(r));
+  return r;
+}
 #else
 __constant__ Dev g_hived_dev;
 #endif
@@ -122,6 +134,8 @@ enum { CMD_IDLE = 0, CMD_VIEW = 1, CMD_EXIT = 2 };
 struct Core {
 #if defined(HIVED_DEV_IN_CONSTANT) && defined(HIVED_MANY_BUILD)
 #define d g_hived_devs[blockIdx.y]  /* (until the end of this header) */
+#elif defined(HIVED_DEV_IN_CONSTANT) && defined(HIVED_CONC_BUILD)
+#define d g_hived_devs[hv_slot_base()]  /* (until the end of this header) */
 #elif defined(HIVED_DEV_IN_CONSTANT)
 #define d g_hived_dev  /* (until the end of this header) */
 #else
@@ -3535,7 +3549,7 @@ struct Core {
 #undef lane
 #undef AS
 
-#ifdef HIVED_MANY_BUILD
-}  // namespace many
+#if defined(HIVED_MANY_BUILD) || defined(HIVED_CONC_BUILD)
+}  // namespace many / conc
 #endif
 }  // namespace hived

@@ -11,11 +11,13 @@
 #include <cuda_runtime.h>
 
 #include <mutex>
+#include <unordered_set>
 
 #define HIVED_BK_LAUNCH_MANY 1  // the joint launch below
-#define HIVED_BK_CONCURRENT 1   // concurrent contexts' own resident kernels below
+#define HIVED_BK_CONCURRENT 1   // concurrent contexts' own resident kernels and batches below
 #include "hived_engine.hpp"
 #include "hived_many.h"
+#include "hived_seats.h"
 
 namespace hived {
 
@@ -78,12 +80,60 @@ static bool cudaOk(cudaError_t e, std::string& err, const char* what) {
   return false;
 }
 
+// A resident per-call kernel (bk_run_small): a non-blocking stream of its own, one request slot in mapped host memory
+// and the device staging of the events it runs.
+struct ServeChan {
+  cudaStream_t stream = nullptr;
+  cudaStream_t copyStream = nullptr;     // concurrent kernels: the pool words beyond the slot's window
+  volatile int32_t* slotHost = nullptr;  // cudaHostAlloc(mapped)
+  int32_t* slotDev = nullptr;
+  hived_result_t* stageRes = nullptr;
+  uint32_t* dSugg = nullptr;
+  int32_t* dAux = nullptr;
+  int32_t* pool = nullptr;
+  long long poolCap = 0;
+  int seq = 0;
+  int conc = -1;         // -1: hived_serve_kernel on g_hived_dev; else the concurrent slot its hived_serve_conc_kernel reads
+  bool alive = false;    // a serve kernel was launched and has not been seen to exit
+  SeatLedger* seat = nullptr;      // hived_serve_kernel: the device's ledger while the kernel holds a seat there
+  SeatLedger* slotSeat = nullptr;  // concurrent kernels: the seat held from creation to destruction
+  long long served = 0, launches = 0;
+  std::vector<void*> retired;  // concurrent batches: cudaMalloc'd staging replaced by pooled memory, freed at destroy
+};
+
+// ---- a concurrent context's batch (bk_batch_begin .. bk_batch_end) ------------------------------------------------
+// In between, the calling thread's copies, staging allocations and launches for the context go to the stream of the
+// context's resident kernel (stopped first) and synchronise with that stream only.  cudaMemcpy would run on the legacy
+// default stream, which waits for every blocking stream (the turn-taking contexts' streams), and cudaFree may
+// synchronise the whole device, which waits until every busy concurrent context's resident kernel has gone idle.
+// Staging that grows inside a batch therefore comes from the stream-ordered allocator; the cudaMalloc'd buffer it
+// replaces is kept until the context is destroyed.
+static thread_local ServeChan* t_own = nullptr;
+static std::mutex g_pooledMu;
+static std::unordered_set<void*> g_pooled;  // every live cudaMallocAsync block of bk_alloc
+
 void* bk_alloc(size_t bytes) {
   void* p = nullptr;
+  if (t_own) {
+    if (cudaMallocAsync(&p, bytes ? bytes : 1, t_own->stream) != cudaSuccess) return nullptr;
+    std::lock_guard<std::mutex> lk(g_pooledMu);
+    g_pooled.insert(p);
+    return p;
+  }
   if (cudaMalloc(&p, bytes ? bytes : 1) != cudaSuccess) return nullptr;
   return p;
 }
-void bk_free(void* p) { cudaFree(p); }
+void bk_free(void* p) {
+  if (!p) return;
+  bool pooled;
+  {
+    std::lock_guard<std::mutex> lk(g_pooledMu);
+    pooled = g_pooled.erase(p) > 0;
+  }
+  if (pooled && t_own) cudaFreeAsync(p, t_own->stream);
+  else if (t_own) t_own->retired.push_back(p);
+  else cudaFree(p);  // (for a pooled block: no implicit synchronisation; the context's last batch was synchronised)
+}
 // The copy hooks have no return value (the engine is backend-neutral): the first failure of the calling thread is kept
 // and reported by the next launchProgram / bk_run_small as a platform error (bk_init, i.e. hived_create, starts clean).
 static thread_local cudaError_t g_copyErr = cudaSuccess;
@@ -95,10 +145,21 @@ static int takeCopyError(std::string& err) {
   cudaGetLastError();
   return HIVED_ERR_PLATFORM;
 }
-void bk_h2d(void* dst, const void* src, size_t bytes) { if (bytes) noteCopy(cudaMemcpy(dst, src, bytes, cudaMemcpyHostToDevice)); }
-void bk_d2h(void* dst, const void* src, size_t bytes) { if (bytes) noteCopy(cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost)); }
-void bk_d2d(void* dst, const void* src, size_t bytes) { if (bytes) noteCopy(cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToDevice)); }
-void bk_zero(void* dst, size_t bytes) { if (bytes) noteCopy(cudaMemset(dst, 0, bytes)); }
+static void copy(void* dst, const void* src, size_t bytes, cudaMemcpyKind kind) {
+  if (!bytes) return;
+  if (!t_own) { noteCopy(cudaMemcpy(dst, src, bytes, kind)); return; }
+  cudaError_t ce = cudaMemcpyAsync(dst, src, bytes, kind, t_own->stream);
+  noteCopy(ce == cudaSuccess ? cudaStreamSynchronize(t_own->stream) : ce);
+}
+void bk_h2d(void* dst, const void* src, size_t bytes) { copy(dst, src, bytes, cudaMemcpyHostToDevice); }
+void bk_d2h(void* dst, const void* src, size_t bytes) { copy(dst, src, bytes, cudaMemcpyDeviceToHost); }
+void bk_d2d(void* dst, const void* src, size_t bytes) { copy(dst, src, bytes, cudaMemcpyDeviceToDevice); }
+void bk_zero(void* dst, size_t bytes) {
+  if (!bytes) return;
+  if (!t_own) { noteCopy(cudaMemset(dst, 0, bytes)); return; }
+  cudaError_t ce = cudaMemsetAsync(dst, 0, bytes, t_own->stream);
+  noteCopy(ce == cudaSuccess ? cudaStreamSynchronize(t_own->stream) : ce);
+}
 
 void bk_flush_l2() {  // one buffer per device (the current one)
   static void* bufs[64] = {nullptr};
@@ -136,24 +197,6 @@ int bk_init(int& device, std::string& err) {
   return 0;
 }
 
-// A resident per-call kernel (bk_run_small): a non-blocking stream of its own, one request slot in mapped host memory
-// and the device staging of the events it runs.
-struct ServeChan {
-  cudaStream_t stream = nullptr;
-  cudaStream_t copyStream = nullptr;     // concurrent kernels: the pool words beyond the slot's window
-  volatile int32_t* slotHost = nullptr;  // cudaHostAlloc(mapped)
-  int32_t* slotDev = nullptr;
-  hived_result_t* stageRes = nullptr;
-  uint32_t* dSugg = nullptr;
-  int32_t* dAux = nullptr;
-  int32_t* pool = nullptr;
-  long long poolCap = 0;
-  int seq = 0;
-  int conc = -1;         // -1: hived_serve_kernel on g_hived_dev; else the concurrent slot its hived_serve_many_kernel reads
-  bool alive = false;    // a serve kernel was launched and has not been seen to exit
-  long long served = 0, launches = 0;
-};
-
 struct CudaTimers {
   cudaEvent_t start = nullptr, stop = nullptr;
   cudaStream_t stream = nullptr;
@@ -167,6 +210,28 @@ static bool noResident() {
   return off && *off && *off != '0';
 }
 
+// ---- co-residency seats (hived_seats.h): one ledger per device, as many seats as CTAs of the program fit on it --------
+static SeatLedger g_seats[64];
+static SeatLedger& seatsOf(const Engine& e) {  // the context's device is current
+  const int dv = e.deviceOrdinal >= 0 && e.deviceOrdinal < 64 ? e.deviceOrdinal : 0;
+  const int fit = manyCoResident(e.deviceOrdinal);
+  if (fit > 0) g_seats[dv].setCapacity(fit);  // (unset while it cannot be queried: every request is refused)
+  return g_seats[dv];
+}
+static int seatError(Engine& e, int n) {
+  char buf[160];
+  snprintf(buf, sizeof buf, "cannot hold %d co-resident CTAs: the device fits %d (occupancy x SMs)", n, seatsOf(e).capacity());
+  e.err = buf;
+  return HIVED_ERR_PLATFORM;
+}
+
+// A resident kernel was seen to exit (or cannot be waited for any more): its seat, if it holds one, is free again.
+static void serveLeft(ServeChan& c) {
+  c.alive = false;
+  if (c.seat) c.seat->release(1);
+  c.seat = nullptr;
+}
+
 // Stop a resident kernel (if any) and wait until it has left.
 static void serveStop(ServeChan& c) {
   if (!c.alive) return;
@@ -177,7 +242,7 @@ static void serveStop(ServeChan& c) {
     s[0] = ++c.seq;
   }
   cudaStreamSynchronize(c.stream);
-  c.alive = false;
+  serveLeft(c);
 }
 
 // ---- whose Dev is in the constant bank (g_hived_dev, hived_core.h) of each device ---------------------------------
@@ -189,6 +254,18 @@ static void serveStop(ServeChan& c) {
 // it (bk_quiesce), since another thread's stop would race with that caller's call in flight.
 static std::recursive_mutex g_devMu;
 static Engine* g_devOwner[64] = {nullptr};
+
+// g_devMu held on behalf of the listed contexts: each one's turn counter (hived_bench_turns) counts the outermost hold
+static thread_local int t_turnDepth = 0;
+struct Turn {
+  std::lock_guard<std::recursive_mutex> lk;
+  Turn(Engine* const* es, int k) : lk(g_devMu) {
+    if (t_turnDepth++ == 0)
+      for (int y = 0; y < k; y++) es[y]->turns++;
+  }
+  explicit Turn(Engine& e) : lk(g_devMu) { if (t_turnDepth++ == 0) e.turns++; }
+  ~Turn() { t_turnDepth--; }
+};
 
 static int ensureDevLoaded(Engine& e) {  // g_devMu held, the context's device current
   const int dv = e.deviceOrdinal >= 0 && e.deviceOrdinal < 64 ? e.deviceOrdinal : 0;
@@ -203,7 +280,7 @@ static int ensureDevLoaded(Engine& e) {  // g_devMu held, the context's device c
 static void concClose(Engine& e);
 void bk_forget(Engine& e) {  // the context is going away
   {
-    std::lock_guard<std::recursive_mutex> lk(g_devMu);
+    Turn turn(e);
     for (auto& o : g_devOwner) if (o == &e) o = nullptr;
   }
   concClose(e);
@@ -212,7 +289,7 @@ void bk_forget(Engine& e) {  // the context is going away
 // Stop the context's resident kernels (if any) and wait until they have left: before anything else launches on or
 // writes to the scheduler state.  Called by the context's own caller, with the context's device current.
 void bk_quiesce(Engine& e) {
-  std::lock_guard<std::recursive_mutex> lk(g_devMu);
+  Turn turn(e);
   CudaTimers* t = (CudaTimers*)e.stream;
   if (!t) return;
   serveStop(t->serve);
@@ -221,12 +298,14 @@ void bk_quiesce(Engine& e) {
 
 // ---- concurrent contexts (HIVED_OPT_CONCURRENT) --------------------------------------------------------------------
 // Each holds one of the device's HIVED_CONCURRENT_MAX slots from hived_create to hived_destroy: its Dev sits in constant
-// slot HIVED_MANY_MAX + s of the joint build (hived_cuda_many.cu), copied once, and its per-call path runs on a resident
-// kernel of its own (hived_serve_many_kernel) through a request slot of its own, without g_devMu.
+// slot s of the concurrent build (hived_cuda_conc.cu), copied once, and its per-call path runs on a resident kernel of
+// its own (hived_serve_conc_kernel) through a request slot of its own, without g_devMu.
 // Invariant: a slot's Dev is written only while no kernel that reads that slot runs (the slot is free: the previous
 // holder's kernel was stopped before it gave the slot back), and the kernel that reads it is launched after the write
 // has completed.  Writes to other slots — another context's creation, a joint launch's slots 0..k-1 — may happen while
-// resident kernels run.
+// resident kernels run.  Taking a slot happens under g_devMu: a g_devMu holder that budgets for the slots in use (the
+// joint launch's rounds) sees no new one appear before it has launched.  Each slot with a resident kernel holds one
+// seat of the device's ledger from creation to destruction.
 static std::mutex g_concMu;
 static Engine* g_concSlot[64][HIVED_CONCURRENT_MAX] = {};
 
@@ -259,6 +338,7 @@ static bool serveAlloc(const Engine& e, ServeChan& c) {
 
 static void serveFree(ServeChan& c) {  // the kernel has left
   cudaFree(c.stageRes); cudaFree(c.dSugg); cudaFree(c.dAux); cudaFree(c.pool);
+  for (void* p : c.retired) cudaFree(p);
   if (c.slotHost) cudaFreeHost((void*)c.slotHost);
   if (c.copyStream) cudaStreamDestroy(c.copyStream);
   if (c.stream) cudaStreamDestroy(c.stream);
@@ -272,6 +352,7 @@ int bk_open_concurrent(Engine& e) {  // the end of hived_create: the device is c
   const int dv = e.deviceOrdinal >= 0 && e.deviceOrdinal < 64 ? e.deviceOrdinal : 0;
   const int fit = manyCoResident(e.deviceOrdinal);
   const int cap = fit - COOP_CTAS_MAX < HIVED_CONCURRENT_MAX ? fit - COOP_CTAS_MAX : HIVED_CONCURRENT_MAX;
+  Turn turn(e);
   int slot = -1;
   {
     std::lock_guard<std::mutex> lk(g_concMu);
@@ -294,6 +375,8 @@ int bk_open_concurrent(Engine& e) {  // the end of hived_create: the device is c
   ServeChan* c = new ServeChan();
   c->conc = slot;
   t->conc = c;
+  if (!seatsOf(e).acquire(1)) return seatError(e, 1);
+  c->slotSeat = &seatsOf(e);
   if (!serveAlloc(e, *c) || cudaStreamCreateWithFlags(&c->copyStream, cudaStreamNonBlocking) != cudaSuccess) {
     e.err = "out of device or pinned host memory for the concurrent context's resident kernel";
     return HIVED_ERR_CAPACITY;
@@ -308,6 +391,7 @@ static void concClose(Engine& e) {  // bk_quiesce has stopped the kernel
   CudaTimers* t = (CudaTimers*)e.stream;
   if (t && t->conc) {
     serveFree(*t->conc);
+    if (t->conc->slotSeat) t->conc->slotSeat->release(1);
     delete t->conc;
     t->conc = nullptr;
   }
@@ -318,8 +402,12 @@ static void concClose(Engine& e) {  // bk_quiesce has stopped the kernel
 
 static_assert(NT / 32 <= MAX_WARPS, "the shared counters are sized for MAX_WARPS warps per CTA");
 
+static int concLaunch(Engine& e, ServeChan& c, int n);
+
 int launchProgram(Engine& e, int n, bool withInit) {
-  std::lock_guard<std::recursive_mutex> lk(g_devMu);
+  // a concurrent context's batch: its own stream, constant slot and seats, no turn
+  if (t_own && e.stream && t_own == ((CudaTimers*)e.stream)->conc && !withInit && !e.mgMode) return concLaunch(e, *t_own, n);
+  Turn turn(e);
   if (!e.stream) {
     // the kernel wants L1, not shared memory: ask for the smallest carveout that holds its ~18 KB of static smem
     cudaFuncSetAttribute(hived_events_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 10);
@@ -334,6 +422,9 @@ int launchProgram(Engine& e, int n, bool withInit) {
   if (int rc = takeCopyError(e.err)) return rc;  // a staging copy of this batch (or of create()) failed
   if (int rc = ensureDevLoaded(e)) return rc;
   const int mgMode = withInit ? 0 : e.mgMode;
+  const int C = withInit ? 1 : (mgMode == 3 ? 1 : e.launchCta);
+  SeatHold seats(seatsOf(e), C);  // until the stream synchronise below has seen the kernels finish
+  if (!seats.ok()) return seatError(e, C);
   if (mgMode == 3) {  // end of a multi-GPU partition run: the repair pass alone
     hived_repair_kernel<<<1, NT, 0, t->stream>>>();
     cudaError_t err = cudaStreamSynchronize(t->stream);
@@ -341,7 +432,6 @@ int launchProgram(Engine& e, int n, bool withInit) {
     e.kernelLaunches++;
     return 0;
   }
-  const int C = withInit ? 1 : e.launchCta;
   long long scal[MAX_CTAS * 4] = {0};
   for (int c = 0; c < C; c++) {
     scal[c * 4 + 0] = withInit ? 0 : (mgMode ? e.mgPoolCur[c] : e.poolBase[c]);
@@ -399,6 +489,56 @@ int launchProgram(Engine& e, int n, bool withInit) {
   return 0;
 }
 
+// A concurrent context's staged batch (bk_batch_begin): the concurrent build's events kernel on the context's constant slot,
+// one CTA per VC group, on the context's own stream.  No g_devMu, no g_hived_dev; the seats of its CTAs are held until
+// the stream synchronise has seen the kernels finish.
+static int concLaunch(Engine& e, ServeChan& c, int n) {
+  CudaTimers* t = (CudaTimers*)e.stream;
+  if (int rc = takeCopyError(e.err)) return rc;  // a staging copy of this batch failed
+  const int C = e.launchCta;
+  long long scal[MAX_CTAS * 4] = {0};
+  for (int k = 0; k < C; k++) { scal[k * 4 + 0] = e.poolBase[k]; scal[k * 4 + 1] = e.poolBase[k + 1]; }
+  const ManySlot q{(const hived_event_t*)e.dEvents.p, (hived_result_t*)e.dResults.p,
+                   e.hasSugg ? (const uint32_t*)e.dSugg.p : nullptr, (int32_t*)e.dPool.p, (long long*)e.dScalars.p,
+                   C > 1 ? (const int32_t*)e.dOwn.p : nullptr, n, C, e.nPinnedOrder, e.nBad};
+  SeatHold seats(seatsOf(e), C);
+  if (!seats.ok()) return seatError(e, C);
+  cudaMemcpyAsync(e.dScalars.p, scal, sizeof scal, cudaMemcpyHostToDevice, c.stream);
+  cudaEventRecord(t->start, c.stream);
+  cudaError_t err = concBatchLaunch(c.conc, q, c.stream);
+  if (err != cudaSuccess) {
+    cudaStreamSynchronize(c.stream);
+    cudaGetLastError();
+    e.err = std::string("launching hived_events_conc_kernel failed: ") + cudaGetErrorString(err);
+    return HIVED_ERR_PLATFORM;
+  }
+  cudaEventRecord(t->stop, c.stream);
+  cudaMemcpyAsync(scal, e.dScalars.p, sizeof scal, cudaMemcpyDeviceToHost, c.stream);
+  err = cudaStreamSynchronize(c.stream);
+  if (err != cudaSuccess || (err = cudaGetLastError()) != cudaSuccess) {
+    e.err = std::string("hived_events_conc_kernel failed: ") + cudaGetErrorString(err);
+    return HIVED_ERR_PLATFORM;
+  }
+  float ms = 0.f;
+  cudaEventElapsedTime(&ms, t->start, t->stop);
+  e.lastKernelMs = ms;
+  e.kernelMsTotal += ms;
+  e.kernelLaunches += C > 1 ? 2 : 1;
+  e.poolEnd.assign(C, 0);
+  for (int k = 0; k < C; k++) e.poolEnd[k] = scal[k * 4 + 0];
+  e.poolOff = scal[0];
+  return 0;
+}
+
+bool bk_batch_begin(Engine& e) {
+  CudaTimers* t = (CudaTimers*)e.stream;
+  if (!t || !t->conc) return false;  // an ordinary context, or HIVED_NO_RESIDENT=1: the batch takes turns
+  serveStop(*t->conc);               // only the context's own caller stops its kernel
+  t_own = t->conc;
+  return true;
+}
+void bk_batch_end(Engine&) { t_own = nullptr; }
+
 // ---- joint launches (include/hived_multictx.h, hived_cuda_many.cu) ------------------------------------------------
 // The staged batches of several contexts of one device run in one launch, each context on CTAs of its own, on the first
 // context's stream.  g_hived_dev and its owner are not touched; but every resident per-call kernel of the device is
@@ -406,7 +546,7 @@ int launchProgram(Engine& e, int n, bool withInit) {
 // may need to have all its CTAs resident).  Contexts whose CTAs do not fit on the device together go to further
 // launches (rounds), greedily in list order.
 int bk_launch_many(Engine* const* es, int k) {
-  std::lock_guard<std::recursive_mutex> lk(g_devMu);
+  Turn turn(es, k);
   Engine& e0 = *es[0];
   const int dv = e0.deviceOrdinal >= 0 && e0.deviceOrdinal < 64 ? e0.deviceOrdinal : 0;
   for (int y = 0; y < k; y++) bk_quiesce(*es[y]);
@@ -435,8 +575,10 @@ int bk_launch_many(Engine* const* es, int k) {
                          C > 1 ? (const int32_t*)e.dOwn.p : nullptr, e.stagedN, C, e.nPinnedOrder, e.nBad};
     devs[y] = &e.dev;
   }
-  cudaEventRecord(t->start, t->stream);
-  for (int y0 = 0; y0 < k;) {  // one round: the longest prefix of the rest whose (widest C) x (count) fits
+  // rounds: the longest prefix of the rest whose (widest C) x (count) fits; they run one after another on one stream,
+  // so the seats of the largest round cover them all
+  int ends[HIVED_MANY_MAX], nRounds = 0, seatsNeeded = 0;
+  for (int y0 = 0; y0 < k;) {
     int y1 = y0 + 1, cmax = a.slot[y0].C;
     while (y1 < k) {
       const int c = a.slot[y1].C > cmax ? a.slot[y1].C : cmax;
@@ -444,11 +586,19 @@ int bk_launch_many(Engine* const* es, int k) {
       cmax = c;
       y1++;
     }
+    if (cmax * (y1 - y0) > seatsNeeded) seatsNeeded = cmax * (y1 - y0);
+    ends[nRounds++] = y1;
+    y0 = y1;
+  }
+  SeatHold seats(seatsOf(e0), seatsNeeded);  // until the stream synchronise below has seen the last round finish
+  if (!seats.ok()) { seatError(e0, seatsNeeded); return fail(e0.err); }
+  cudaEventRecord(t->start, t->stream);
+  for (int i = 0, y0 = 0; i < nRounds; y0 = ends[i++]) {
+    const int y1 = ends[i];
     ManyArgs r;
     for (int y = y0; y < y1; y++) r.slot[y - y0] = a.slot[y];
     cudaError_t le = manyLaunch(devs + y0, r, y1 - y0, t->stream);
     if (le != cudaSuccess) { cudaStreamSynchronize(t->stream); cudaGetLastError(); return fail(std::string("joint launch failed: ") + cudaGetErrorString(le)); }
-    y0 = y1;
   }
   cudaEventRecord(t->stop, t->stream);
   for (int y = 0; y < k; y++)
@@ -525,32 +675,37 @@ static int serveCall(Engine& e, ServeChan& c, const hived_event_t* events, int n
     // 1500 polls over PCIe: the kernel leaves after 1.5-2 ms without a request on an H100
     // (profiles/micro/resident_idle_timeout.py)
     cudaError_t le = cudaSuccess;
-    if (c.conc < 0)
+    if (c.conc < 0) {
+      // it stays resident after g_devMu is released: it holds a seat until it is seen to leave (serveLeft)
+      if (!c.seat) {
+        if (!seatsOf(e).acquire(1)) { seatError(e, 1); return false; }
+        c.seat = &seatsOf(e);
+      }
       hived_serve_kernel<<<1, NT, 0, c.stream>>>(c.slotDev, seq - 1, 1500, c.stageRes, c.dSugg, c.dAux, e.nPinnedOrder, e.nBad,
                                                  c.pool);
-    else
+    } else
       le = concServeLaunch(c.conc, c.slotDev, seq - 1, 1500, c.stageRes, c.dSugg, c.dAux, e.nPinnedOrder, e.nBad, c.pool, c.stream);
-    if (le != cudaSuccess) { e.err = std::string("launching hived_serve_many_kernel failed: ") + cudaGetErrorString(le); return false; }
+    if (le != cudaSuccess) { e.err = std::string("launching hived_serve_conc_kernel failed: ") + cudaGetErrorString(le); return false; }
     c.alive = true;
     c.launches++;
     e.kernelLaunches++;
     return true;
   };
-  if (!c.alive && !launch()) return HIVED_ERR_PLATFORM;
+  if (!c.alive && !launch()) { serveLeft(c); return HIVED_ERR_PLATFORM; }
   // wait for `done`; a kernel that left just before the request arrived is replaced
   long long spins = 0;
   while (s[SERVE_DONE_OFF] != seq) {
     if (s[SERVE_DONE_OFF + 4] && s[SERVE_DONE_OFF] != seq) {
       cudaError_t err = cudaStreamSynchronize(c.stream);
-      if (err != cudaSuccess) { e.err = std::string("hived_serve_kernel failed: ") + cudaGetErrorString(err); c.alive = false; return HIVED_ERR_PLATFORM; }
+      if (err != cudaSuccess) { e.err = std::string("hived_serve_kernel failed: ") + cudaGetErrorString(err); serveLeft(c); return HIVED_ERR_PLATFORM; }
       if (s[SERVE_DONE_OFF] == seq) break;
-      if (!launch()) { c.alive = false; return HIVED_ERR_PLATFORM; }
+      if (!launch()) { serveLeft(c); return HIVED_ERR_PLATFORM; }
     }
     if ((++spins & 0xfffff) == 0) {  // every ~million polls: is the kernel still healthy?
       cudaError_t err = cudaStreamQuery(c.stream);
       if (err != cudaSuccess && err != cudaErrorNotReady) {
         e.err = std::string("hived_serve_kernel failed: ") + cudaGetErrorString(err);
-        c.alive = false;
+        serveLeft(c);
         return HIVED_ERR_PLATFORM;
       }
     }
@@ -588,15 +743,20 @@ int bk_run_small(Engine& e, const hived_event_t* events, int n, const uint32_t* 
   if (!e.stream) return -1;  // the first launch (initialisation) creates the stream
   CudaTimers* t = (CudaTimers*)e.stream;
   const bool takes = serveTakes(n, suggPool, suggWords, aux, auxWords);
-  // a concurrent context: its own resident kernel and constant slot, no g_devMu, no turn on g_hived_dev
+  // a concurrent context: its own resident kernel and constant slot, no g_devMu, no turn on g_hived_dev.  A call its
+  // kernel does not take runs as a batch of its own (bk_batch_begin), except one with aux words (bind info over
+  // SERVE_AUX_MAX, only ever a single hived_add_allocated_pod): the concurrent build's events kernel takes the joint
+  // launch's ManySlot, which carries none, so that one takes turns.
+  const bool hasAux = aux != nullptr && auxWords > 0;
   if (t->conc && takes) return serveCall(e, *t->conc, events, n, suggPool, suggWords, aux, auxWords, res, pool, poolCap);
-  std::lock_guard<std::recursive_mutex> lk(g_devMu);
-  if (t->conc) serveStop(*t->conc);  // (a call its kernel does not take) the launch below writes the same state
+  if (t->conc && !hasAux) return -1;
+  Turn turn(e);
+  if (t->conc) serveStop(*t->conc);  // the launch below writes the same state
   if (int rc = ensureDevLoaded(e)) return rc;
   if (!t->conc && takes && serveSetup(e, t))
     return serveCall(e, t->serve, events, n, suggPool, suggWords, aux, auxWords, res, pool, poolCap);
   static thread_local SmallStage stage;  // per host thread; the shim serialises calls per context anyway
-  const bool hasSugg = suggPool != nullptr && suggWords > 0, hasAux = aux != nullptr && auxWords > 0;
+  const bool hasSugg = suggPool != nullptr && suggWords > 0;
   const int64_t window = poolCap < SMALL_POOL_WINDOW ? poolCap : SMALL_POOL_WINDOW;
   const size_t oEv = 0, oScal = oEv + (size_t)n * sizeof(hived_event_t), oSugg = oScal + 4 * sizeof(long long),
                oAux = oSugg + (hasSugg ? (size_t)suggWords * 4 : 0), oRes = (oAux + (hasAux ? (size_t)auxWords * 4 : 0) + 15) & ~(size_t)15,
@@ -747,19 +907,20 @@ int bk_canonicalise(Engine& e, int n, long long* total) {
   *total = 0;
   if (n <= 0) return 0;
   CudaTimers* t = (CudaTimers*)e.stream;
+  cudaStream_t st = t_own ? t_own->stream : t->stream;  // a concurrent context's batch: its own stream
   const int nb = (n + SCAN_BLOCK - 1) / SCAN_BLOCK;
   e.dScan.ensure((size_t)n * 4 + (size_t)(nb + 2) * 8 + 16);
   long long* blockSum = (long long*)e.dScan.p;              // [nb + 1], 8-byte aligned at the front
   int32_t* excl = (int32_t*)((char*)e.dScan.p + (size_t)(nb + 2) * 8);
   e.dPool2.ensure((size_t)(e.poolCapWords > 0 ? e.poolCapWords : 1) * 4);
   if (e.buffersFailed()) { e.err = "out of device memory for the pool compaction"; return HIVED_ERR_CAPACITY; }
-  pool_words_kernel<<<nb, SCAN_T, 0, t->stream>>>((const hived_result_t*)e.dResults.p, n, excl, blockSum);
-  pool_block_scan_kernel<<<1, 1024, 0, t->stream>>>(blockSum, nb);
-  pool_gather_kernel<<<(int)(((long long)n * 32 + 255) / 256), 256, 0, t->stream>>>((hived_result_t*)e.dResults.p, n, excl, blockSum,
+  pool_words_kernel<<<nb, SCAN_T, 0, st>>>((const hived_result_t*)e.dResults.p, n, excl, blockSum);
+  pool_block_scan_kernel<<<1, 1024, 0, st>>>(blockSum, nb);
+  pool_gather_kernel<<<(int)(((long long)n * 32 + 255) / 256), 256, 0, st>>>((hived_result_t*)e.dResults.p, n, excl, blockSum,
                                                                               (const int32_t*)e.dPool.p, (int32_t*)e.dPool2.p);
   long long tot = 0;
-  cudaMemcpyAsync(&tot, blockSum + nb, 8, cudaMemcpyDeviceToHost, t->stream);
-  cudaError_t err = cudaStreamSynchronize(t->stream);
+  cudaMemcpyAsync(&tot, blockSum + nb, 8, cudaMemcpyDeviceToHost, st);
+  cudaError_t err = cudaStreamSynchronize(st);
   if (err != cudaSuccess || (err = cudaGetLastError()) != cudaSuccess) {
     e.err = std::string("pool compaction failed: ") + cudaGetErrorString(err);
     return HIVED_ERR_PLATFORM;

@@ -1,6 +1,5 @@
 // libhived_cuda.so, second translation unit: the device program of hived_core.h built once more for joint launches
-// (include/hived_multictx.h) and for the resident per-call kernels of concurrent contexts (HIVED_OPT_CONCURRENT,
-// include/hived.h).  The only difference from hived_cuda.cu's build is where a CTA finds the scheduler state: its
+// (include/hived_multictx.h).  The only difference from hived_cuda.cu's build is where a CTA finds the scheduler state: its
 // context's Dev sits in constant slot blockIdx.y (g_hived_devs[blockIdx.y]) instead of the single g_hived_dev, so the
 // kernels of hived_cuda.cu — and the turn-taking of single-context calls around g_hived_dev — stay exactly as they are.
 #define HIVED_MANY_BUILD 1
@@ -44,25 +43,6 @@ __global__ void __launch_bounds__(NT, 1) hived_repair_many_kernel(const __grid_c
   core.repairSharedAncestors();
 }
 
-// The resident per-call kernel of a concurrent context (HIVED_OPT_CONCURRENT): hived_serve_kernel of hived_cuda.cu, with
-// the context's Dev in constant slot HIVED_MANY_MAX + s.  Launched on a grid (1, HIVED_MANY_MAX + s + 1): the last row
-// is the context's CTA, every other CTA returns at once.
-__global__ void __launch_bounds__(NT, 1)
-hived_serve_many_kernel(volatile int32_t* slot, int seq0, int idleSpins, hived_result_t* stageRes, uint32_t* dSugg,
-                        int32_t* dAux, int nPinnedOrder, int nBad, int32_t* pool) {
-  if (blockIdx.y != gridDim.y - 1) return;
-  Sm& sm = g_hived_sm;
-  if (threadIdx.x == 0) {
-    sm.cmd = CMD_IDLE;
-    sm.panic = 0;
-    sm.lead_k = 0x7fffffff;
-    sm.pool_off = 0;
-  }
-  __syncthreads();
-  Core core(g_hived_devs[blockIdx.y], &sm, pool, 0, 1);
-  core.serve(slot, seq0, idleSpins, stageRes, dSugg, dAux, nPinnedOrder, nBad);
-}
-
 }  // namespace many
 
 int manyCoResident(int device) {
@@ -95,18 +75,6 @@ cudaError_t manyLaunch(const Dev* const* devs, const ManyArgs& a, int k, cudaStr
   if (e != cudaSuccess) return e;
   if (parallel) e = cudaLaunchKernel((const void*)many::hived_repair_many_kernel, dim3(1, k), dim3(many::NT), args, 0, st);
   return e;
-}
-
-cudaError_t concLoadDev(const Dev& dev, int s, cudaStream_t st) {
-  cudaFuncSetAttribute(many::hived_serve_many_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 10);
-  return cudaMemcpyToSymbolAsync(many::g_hived_devs, &dev, sizeof(Dev), (size_t)(HIVED_MANY_MAX + s) * sizeof(Dev),
-                                 cudaMemcpyHostToDevice, st);
-}
-
-cudaError_t concServeLaunch(int s, volatile int32_t* slot, int seq0, int idleSpins, hived_result_t* stageRes, uint32_t* dSugg,
-                            int32_t* dAux, int nPinnedOrder, int nBad, int32_t* pool, cudaStream_t st) {
-  void* args[] = {&slot, &seq0, &idleSpins, &stageRes, &dSugg, &dAux, &nPinnedOrder, &nBad, &pool};
-  return cudaLaunchKernel((const void*)many::hived_serve_many_kernel, dim3(1, HIVED_MANY_MAX + s + 1), dim3(many::NT), args, 0, st);
 }
 
 }  // namespace hived

@@ -53,6 +53,11 @@ int bk_launch_many(Engine* const* es, int k);
 // own (0, or HIVED_ERR_* with err set).  A backend that defines HIVED_BK_CONCURRENT supplies it; the others accept the
 // flag and ignore it.
 int bk_open_concurrent(Engine& e);
+// a batch of such a context that the per-call path does not take: between bk_batch_begin (true) and bk_batch_end the
+// calling thread's copies, staging allocations and launches for it synchronise with nothing but the context's own
+// work.  false: the batch takes turns as every other context's does.  Supplied with HIVED_BK_CONCURRENT, as above.
+bool bk_batch_begin(Engine& e);
+void bk_batch_end(Engine& e);
 void bk_flush_l2();
 
 struct Buf {
@@ -105,6 +110,7 @@ struct Engine {
   float lastKernelMs = 0.f;
   double kernelMsTotal = 0.0;
   long long kernelLaunches = 0;
+  long long turns = 0;  // calls that took the backend's device lock for this context (hived_bench_turns)
   void* stream = nullptr;
 
   ~Engine() {
@@ -380,6 +386,12 @@ struct Engine {
       int rc = bk_run_small(*this, events, n, suggPool, suggWords, aux, auxWords, res, pool, poolCap);
       if (rc >= 0) { if (rc == 0) trackHealth(events, n); return rc; }
     }
+    struct Own {  // a concurrent context's batch runs on its own (bk_batch_begin)
+      Engine& e;
+      const bool on;
+      explicit Own(Engine& x) : e(x), on(bk_batch_begin(x)) {}
+      ~Own() { if (on) bk_batch_end(e); }
+    } own(*this);
     int rc = stageBatch(events, n, suggPool, suggWords, aux, auxWords, poolCap);
     if (rc) return rc;
     rc = launchProgram(*this, n, false);
@@ -682,6 +694,8 @@ int bk_launch_many(Engine* const* es, int k) {
 #endif
 #ifndef HIVED_BK_CONCURRENT
 int bk_open_concurrent(Engine&) { return 0; }
+bool bk_batch_begin(Engine&) { return false; }
+void bk_batch_end(Engine&) {}
 #endif
 
 }  // namespace hived
@@ -1184,6 +1198,7 @@ uint64_t hived_debug_bookkeeping_hash(hived_ctx* ctx) {
 double hived_bench_last_kernel_ms(hived_ctx* ctx) { return ctx->e.lastKernelMs; }
 double hived_bench_total_kernel_ms(hived_ctx* ctx) { return ctx->e.kernelMsTotal; }
 int64_t hived_bench_kernel_launches(hived_ctx* ctx) { return ctx->e.kernelLaunches; }
+int64_t hived_bench_turns(hived_ctx* ctx) { return ctx->e.turns; }
 
 }  // extern "C"
 

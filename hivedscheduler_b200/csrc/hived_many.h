@@ -1,6 +1,7 @@
-// Joint launches (include/hived_multictx.h): the interface between hived_cuda.cu (host side, one stream, the per-context
-// staging and bookkeeping) and hived_cuda_many.cu (the second build of the device program, which reads context y's Dev
-// from constant slot y).
+// Joint launches (include/hived_multictx.h) and concurrent contexts (HIVED_OPT_CONCURRENT): the interface between
+// hived_cuda.cu (host side: streams, the per-context staging and bookkeeping) and the other two builds of the device
+// program: hived_cuda_many.cu, which reads context y's Dev from constant slot y, and hived_cuda_conc.cu, which reads
+// concurrent slot s's Dev from its constant slot s (the launch's dynamic shared-memory byte count names s).
 #pragma once
 #include <cuda_runtime.h>
 
@@ -30,12 +31,15 @@ int manyCoResident(int device);
 // the joint repair kernel for those contexts.  Everything is queued on `st`; the caller synchronises.
 cudaError_t manyLaunch(const Dev* const* devs, const ManyArgs& a, int k, cudaStream_t st);
 
-// concurrent contexts (HIVED_OPT_CONCURRENT): concurrent slot s (0 <= s < HIVED_CONCURRENT_MAX) is constant slot
-// HIVED_MANY_MAX + s.  concLoadDev queues the copy of the context's Dev into it on `st`; the caller synchronises before
+// concurrent contexts (HIVED_OPT_CONCURRENT, hived_cuda_conc.cu): concurrent slot s (0 <= s < HIVED_CONCURRENT_MAX) is
+// constant slot s of that build.  concLoadDev queues the copy of the context's Dev into it on `st`; the caller synchronises before
 // the first launch.  concServeLaunch queues the slot's resident per-call kernel (Core::serve, arguments as for
 // hived_serve_kernel) on `st`.
 cudaError_t concLoadDev(const Dev& dev, int s, cudaStream_t st);
 cudaError_t concServeLaunch(int s, volatile int32_t* slot, int seq0, int idleSpins, hived_result_t* stageRes, uint32_t* dSugg,
                             int32_t* dAux, int nPinnedOrder, int nBad, int32_t* pool, cudaStream_t st);
+// concBatchLaunch queues one batch of the context in concurrent slot s (q, whose C CTAs run it) on `st`: the events
+// kernel on C CTAs, cooperatively when C > 1, then the repair kernel when C > 1.  The caller synchronises.
+cudaError_t concBatchLaunch(int s, const ManySlot& q, cudaStream_t st);
 
 }  // namespace hived

@@ -626,6 +626,12 @@ class BatchContext:
     def result_hash(self) -> int:
         return int(self.lib.hived_result_hash(self.ctx))
 
+    def turns(self) -> int:
+        """hived_bench_turns (include/hived_bench.h): this context's calls that took turns on the library's device lock."""
+        fn = self.lib.hived_bench_turns
+        fn.restype, fn.argtypes = C.c_int64, [C.c_void_p]
+        return int(fn(self.ctx))
+
     def stats(self) -> Dict[str, int]:
         st = _cabi.Stats()
         self.lib.hived_get_stats(self.ctx, C.byref(st))

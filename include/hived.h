@@ -13,19 +13,24 @@
  *   different threads; contexts that live on the same GPU take turns there (the device-side view of a context's state
  *   sits in the device's constant bank, one context at a time: a process-wide lock inside the library).  To run the
  *   batches of several contexts on one GPU at the same time, hand them to one call: hived_multictx.h.
- *   A context created with HIVED_OPT_CONCURRENT in hived_options_t.flags does not take turns for its per-call path:
- *   hived_schedule, hived_add_allocated_pod, hived_delete_*, hived_set_node_health and hived_process_events of at most 8
- *   events run on a resident kernel of its own, which reads the context's device-side view from a constant slot the
- *   context holds for its whole life.  Such a call waits for no other context's call and stops no other context's
- *   kernel, so each context may be driven by its own thread at the same time as the others, on the same GPU too.  Still
- *   taking turns, with the same answers: its batches of more than 8 events, calls with more than 4096 words of
- *   suggested-node bitmaps, a hived_add_allocated_pod whose bind info and leaves take more than 8192 words, and every
- *   call when HIVED_NO_RESIDENT=1 is set.  A
- *   device holds HIVED_CONCURRENT_MAX such contexts; hived_create of one more returns HIVED_ERR_CAPACITY, creates nothing
- *   and names the limit in hived_create_error().  Cost: each keeps one SM busy while its calls keep coming (its kernel
- *   leaves after ~2 ms without a call and is relaunched on demand).  A device-wide synchronisation elsewhere in the
- *   process (cudaDeviceSynchronize; cudaFree may synchronise too, and hived_destroy and the buffer growth of a large
- *   batch call it) waits until every such kernel has left, i.e. until each busy context pauses its calls for ~2 ms.
+ *   A context created with HIVED_OPT_CONCURRENT in hived_options_t.flags does not take turns: its per-call path
+ *   (hived_schedule, hived_add_allocated_pod, hived_delete_*, hived_set_node_health and hived_process_events of at
+ *   most 8 events) runs on a resident kernel of its own, which reads the context's device-side view from a constant
+ *   slot the context holds for its whole life, and every other hived_process_events and hived_schedule (larger
+ *   batches, more than 4096 words of suggested-node bitmaps) runs as a batch on the context's own stream and CTAs,
+ *   with the same answers.  Such a call waits for no other context's call or batch and stops no other context's
+ *   kernel, so each context may be driven by its own thread at the same time as the others, on the same GPU too; a
+ *   batch only waits until its CTAs can all be resident on the device beside the other contexts' kernels.  Still
+ *   taking turns, with the same answers: hived_create and hived_destroy, joint calls (hived_multictx.h), the
+ *   multi-GPU partition (hived_multigpu.h), the staging and state-rewind hooks of hived_bench.h, a
+ *   hived_add_allocated_pod whose bind info and leaves take more than 8192 words, and every call when
+ *   HIVED_NO_RESIDENT=1 is set.  A device holds HIVED_CONCURRENT_MAX such contexts; hived_create of one more returns
+ *   HIVED_ERR_CAPACITY, creates nothing and names the limit in hived_create_error().  Cost: each keeps one SM busy
+ *   while its calls keep coming (its kernel leaves after ~2 ms without a call and is relaunched on demand).  A
+ *   device-wide synchronisation elsewhere in the process (cudaDeviceSynchronize; cudaFree may synchronise too, and
+ *   hived_destroy and the buffer growth of an ordinary context's large batch call it) waits until every such kernel
+ *   has left, i.e. until each busy context pauses its calls for ~2 ms; a concurrent context's own batches grow their
+ *   buffers without one.
  * Conventions
  *   - plain C, ints and pointers only, no callbacks, nothing retained after a call returns;
  *   - every buffer is caller-owned; results are written into caller-provided arrays;
@@ -143,8 +148,9 @@ typedef struct hived_options {
   int32_t reserved[2];
 } hived_options_t;
 #define HIVED_OPT_NO_RESULT_HASH 1 /* do not maintain hived_result_hash (a parity witness, ~4 CPU cycles per result byte) */
-#define HIVED_OPT_CONCURRENT 2     /* per-call path on a resident kernel of the context's own, driven by its own thread at
-                                      the same time as other contexts of the process (see "Threads" above) */
+#define HIVED_OPT_CONCURRENT 2     /* per-call path on a resident kernel of the context's own and batches on its own
+                                      stream and CTAs, driven by its own thread at the same time as other contexts of the
+                                      process (see "Threads" above) */
 #define HIVED_CONCURRENT_MAX 16    /* HIVED_OPT_CONCURRENT contexts per device */
 
 /* api.PodSchedulingSpec after internal.ExtractPodSchedulingSpec (pkg/api/types.go:78-99,

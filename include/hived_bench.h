@@ -28,6 +28,9 @@ int hived_bench_path_counters(hived_ctx*, int64_t* out);
 double hived_bench_last_kernel_ms(hived_ctx*);   /* CUDA-event time of the last launch, on its stream */
 double hived_bench_total_kernel_ms(hived_ctx*);
 int64_t hived_bench_kernel_launches(hived_ctx*);
+/* calls of this context (hived_create and hived_destroy included) that took the library's process-wide device lock,
+   i.e. took turns with the other contexts of the process (include/hived.h "Threads"); 0 in the host builds */
+int64_t hived_bench_turns(hived_ctx*);
 int hived_bench_num_ctas(hived_ctx*);            /* CTAs the last batch ran on (VC-parallel execution) */
 int hived_bench_set_result_hash(hived_ctx*, int on); /* toggle the running parity hash (HIVED_OPT_NO_RESULT_HASH) */
 #ifdef __cplusplus

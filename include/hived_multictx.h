@@ -13,9 +13,10 @@
  *
  * Concurrent contexts (HIVED_OPT_CONCURRENT, hived.h) may be listed like any other: the call first stops the resident
  * per-call kernel of each listed context (the caller holds it, so none of its calls is in flight) and its next per-call
- * operation starts a new one.  Concurrent contexts that are not listed keep answering their own threads' calls during
- * the joint call; the launch leaves one SM per concurrent context of the device to them, so a list may need one more
- * round than it would on an otherwise idle device.
+ * operation starts a new one.  Concurrent contexts that are not listed keep answering their own threads' calls and
+ * running their batches during the joint call; the launch leaves one SM per concurrent context of the device to them, so
+ * a list may need one more round than it would on an otherwise idle device, and it waits until its largest round's CTAs
+ * can all be resident beside their running batches.
  */
 #ifndef HIVED_MULTICTX_H_
 #define HIVED_MULTICTX_H_
