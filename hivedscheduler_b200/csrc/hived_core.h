@@ -169,6 +169,9 @@ struct Core {
   // cluster (every other CTA of every rank is parked), the cluster-wide state being this rank's to write
   int mgMode = 0, mgStart = 0;
   bool mgStop = false;
+  // the host judged the batch calm (Engine::prepare): the leader runs the calm loop (hived_calm.inc).  From the Dev
+  // (host builds) or from the launch's scalar word 2 (CUDA kernels)
+  bool calm;
   int curEvent;      // index (in the batch) of the event being processed
   bool sharedHeld;   // this event already holds the right to touch the cluster-wide free-list state
 
@@ -181,7 +184,8 @@ struct Core {
         sm_(s_),
 #endif
         sugg(nullptr), pool(pool_), pool_cap(cap), poolOff(0), panicCode(0),
-        s(dev.scratch[hv_cta()]), cta(hv_cta()), nCta(nCta_), multi(nCta_ > 1), curEvent(0), sharedHeld(false), prioMask(0) {
+        s(dev.scratch[hv_cta()]), cta(hv_cta()), nCta(nCta_), multi(nCta_ > 1), calm(dev.calm != 0), curEvent(0), sharedHeld(false),
+        prioMask(0) {
     for (int i = 0; i < N_WORK; i++) work[i] = 0;
     for (int i = 0; i < PC_COUNT; i++) pathCnt[i] = 0;
     if (dev.S.LS <= 64 && dev.S.PS <= 16) {
@@ -1200,6 +1204,7 @@ struct Core {
   // ======================================================================================
 #include "hived_lean.inc"
 #include "hived_runahead.inc"
+#include "hived_calm.inc"
 
   // ======================================================================================
   // cluster-view pass: data-parallel over the CTA
@@ -3405,6 +3410,18 @@ struct Core {
   }
   HIVED_DEV void runLeader(const hived_event_t* events, int n, hived_result_t* results, const uint32_t* suggPool, const int32_t* aux,
                            const int32_t* initLists, int nPinnedOrder, int nBad, const int32_t* own, int nOwn) {
+    if (calm && !initLists && mgMode == 0) runLeaderCalm(events, n, results, suggPool, aux, own, nOwn);
+    else leaderLoop<false>(events, n, results, suggPool, aux, initLists, nPinnedOrder, nBad, own, nOwn);
+  }
+  // the calm loop (hived_calm.inc).  Inlined: as an out-of-line function (one contiguous stretch of code) it reached
+  // the members of Core through `this` and measured 9 % slower (DESIGN.md §4)
+  HIVED_DEV void runLeaderCalm(const hived_event_t* events, int n, hived_result_t* results, const uint32_t* suggPool,
+                                        const int32_t* aux, const int32_t* own, int nOwn) {
+    leaderLoop<true>(events, n, results, suggPool, aux, nullptr, 0, 0, own, nOwn);
+  }
+  template <bool CALM>
+  HIVED_DEV void leaderLoop(const hived_event_t* events, int n, hived_result_t* results, const uint32_t* suggPool, const int32_t* aux,
+                            const int32_t* initLists, int nPinnedOrder, int nBad, const int32_t* own, int nOwn) {
     poolOff = smp()->pool_off;
     int initPanic = 0;
     if (initLists) { initState(initLists, nPinnedOrder, initLists + nPinnedOrder, nBad); initPanic = panicCode; }
@@ -3442,7 +3459,8 @@ struct Core {
       }
       if (k + 2 < nOwn) hv_prefetch(&events[ownAt(k + 2)]);
       dbg(14, tq);
-      processEvent(*reinterpret_cast<const hived_event_t*>(cur), &results[i], suggPool, aux);
+      if constexpr (CALM) calmEvent(*reinterpret_cast<const hived_event_t*>(cur), &results[i], suggPool, aux);
+      else processEvent(*reinterpret_cast<const hived_event_t*>(cur), &results[i], suggPool, aux);
       if (mgStop) { hv_cp_async_wait(); stopK = k; break; }
       tq = pclock();
       if (multi) {

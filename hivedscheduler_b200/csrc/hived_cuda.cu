@@ -24,7 +24,7 @@ namespace hived {
 constexpr int NT = 512;  // threads per CTA (16 warps); the kernel needs the full register file of one SM
 
 // scalars: 4 words per CTA — [0] pool offset (in: start of the CTA's slice, out: first unused word),
-// [1] end of the slice, [2] out: initialisation panic code
+// [1] end of the slice, [2] in: the batch is calm (Core::calm), out: initialisation panic code
 __global__ void __launch_bounds__(NT, 1)
 hived_events_kernel(const hived_event_t* __restrict__ events, int n, hived_result_t* results,
                     const uint32_t* suggPool, const int32_t* aux, const int32_t* initLists, int nPinnedOrder, int nBad,
@@ -43,6 +43,7 @@ hived_events_kernel(const hived_event_t* __restrict__ events, int n, hived_resul
   // multi-GPU partition: [start, limit) of this CTA's list and the mode, packed by launchProgram (0: an ordinary run)
   const long long mg = scalars[cta * 4 + 3];
   if (mg) { core.setMultiGpu((int)((mg >> 62) & 3), (int)(mg & 0x7fffffff)); nOwn = (int)((mg >> 31) & 0x7fffffff); }
+  core.calm = scalars[cta * 4 + 2] != 0;
   core.run(events, n, results, suggPool, aux, initLists, nPinnedOrder, nBad, own ? own + ownOff[cta] : nullptr, nOwn);
   __syncthreads();
   if (threadIdx.x == 0) {
@@ -436,6 +437,7 @@ int launchProgram(Engine& e, int n, bool withInit) {
   for (int c = 0; c < C; c++) {
     scal[c * 4 + 0] = withInit ? 0 : (mgMode ? e.mgPoolCur[c] : e.poolBase[c]);
     scal[c * 4 + 1] = withInit ? 0 : e.poolBase[c + 1];
+    scal[c * 4 + 2] = !withInit && !mgMode && e.dev.calm;
     if (mgMode) scal[c * 4 + 3] = ((long long)mgMode << 62) | ((long long)e.mgLimit[c] << 31) | (long long)e.mgCursor[c];
   }
   cudaMemcpyAsync(e.dScalars.p, scal, sizeof scal, cudaMemcpyHostToDevice, t->stream);
@@ -497,7 +499,7 @@ static int concLaunch(Engine& e, ServeChan& c, int n) {
   if (int rc = takeCopyError(e.err)) return rc;  // a staging copy of this batch failed
   const int C = e.launchCta;
   long long scal[MAX_CTAS * 4] = {0};
-  for (int k = 0; k < C; k++) { scal[k * 4 + 0] = e.poolBase[k]; scal[k * 4 + 1] = e.poolBase[k + 1]; }
+  for (int k = 0; k < C; k++) { scal[k * 4 + 0] = e.poolBase[k]; scal[k * 4 + 1] = e.poolBase[k + 1]; scal[k * 4 + 2] = e.dev.calm; }
   const ManySlot q{(const hived_event_t*)e.dEvents.p, (hived_result_t*)e.dResults.p,
                    e.hasSugg ? (const uint32_t*)e.dSugg.p : nullptr, (int32_t*)e.dPool.p, (long long*)e.dScalars.p,
                    C > 1 ? (const int32_t*)e.dOwn.p : nullptr, n, C, e.nPinnedOrder, e.nBad};
@@ -568,7 +570,7 @@ int bk_launch_many(Engine* const* es, int k) {
     Engine& e = *es[y];
     const int C = e.launchCta;
     long long* s = &scal[(size_t)y * MAX_CTAS * 4];
-    for (int c = 0; c < C; c++) { s[c * 4 + 0] = e.poolBase[c]; s[c * 4 + 1] = e.poolBase[c + 1]; }
+    for (int c = 0; c < C; c++) { s[c * 4 + 0] = e.poolBase[c]; s[c * 4 + 1] = e.poolBase[c + 1]; s[c * 4 + 2] = e.dev.calm; }
     cudaMemcpyAsync(e.dScalars.p, s, MAX_CTAS * 4 * sizeof(long long), cudaMemcpyHostToDevice, t->stream);
     a.slot[y] = ManySlot{(const hived_event_t*)e.dEvents.p, (hived_result_t*)e.dResults.p,
                          e.hasSugg ? (const uint32_t*)e.dSugg.p : nullptr, (int32_t*)e.dPool.p, (long long*)e.dScalars.p,

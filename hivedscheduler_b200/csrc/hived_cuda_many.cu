@@ -27,6 +27,7 @@ __global__ void __launch_bounds__(NT, 1) hived_events_many_kernel(const __grid_c
   Core core(g_hived_devs[blockIdx.y], &sm, q.pool, q.scalars[cta * 4 + 1], q.C);
   const int32_t* ownOff = q.own ? q.own + q.n : nullptr;
   const int nOwn = q.own ? ownOff[cta + 1] - ownOff[cta] : q.n;
+  core.calm = q.scalars[cta * 4 + 2] != 0;
   core.run(q.events, q.n, q.results, q.sugg, nullptr, nullptr, q.nPinnedOrder, q.nBad, q.own ? q.own + ownOff[cta] : nullptr, nOwn);
   __syncthreads();
   if (threadIdx.x == 0) {

@@ -118,6 +118,9 @@ struct Dev {
   int32_t* epoch;          // [MAX_CTAS] per-CTA stamp for vx_stamp
   const Scratch* scratch;  // [nCta] private scratch arrays of every CTA
   int32_t* progress;       // [MAX_CTAS] index of the event each CTA is working on (multi-CTA ordering)
+  // the staged batch runs the calm leader loop (Engine::prepare, hived_calm.inc).  Read from here by the host builds;
+  // the CUDA kernels, whose Dev is a copy in the constant bank, get it in the launch's scalar word 2
+  int32_t calm;
 };
 
 enum {
@@ -132,7 +135,8 @@ enum {
   /* which path the events took (always counted; hived_bench_path_counters) */
   ST_PATH0 = 40, PC_FAST_VIEW = 0 /* scheduling passes answered by the bucketed view */, PC_GENERAL_VIEW = 1 /* full view passes */,
   PC_BK_REBUILD = 2, PC_BK_MOVERS = 3, PC_FAST_COMMIT = 4, PC_GENERAL_COMMIT = 5, PC_FAST_DELETE = 6, PC_GENERAL_DELETE = 7,
-  PC_FAST_MAP = 8, PC_GENERAL_MAP = 9, PC_POD_LEAN = 10, PC_COUNT = 12,
+  PC_FAST_MAP = 8, PC_GENERAL_MAP = 9, PC_POD_LEAN = 10,
+  PC_CALM = 12 /* events the calm loop ran itself */, PC_CALM_FALLBACK = 13 /* events it handed to the general code */, PC_COUNT = 14,
   ST_COUNT = 40 + PC_COUNT
 };
 

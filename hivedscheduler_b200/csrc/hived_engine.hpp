@@ -263,7 +263,9 @@ struct Engine {
     batchStamp++;
     if (groupStamp.size() != groupVcHost.size()) groupStamp.assign(groupVcHost.size(), 0);
     uint64_t mask = prioMaskHost;
-    bool simple = nCtaMax > 1 && n >= 256 && badCount == 0 && !everRecovered;
+    // `calm`: the regime; the batch runs VC-parallel when it is calm and large enough to be split
+    const bool split = nCtaMax > 1 && n >= 256;
+    bool calm = badCount == 0 && !everRecovered;
     // one pass over the events: regime flags, the owner CTA of every event and the pool words every owner may need
     const int C = nCtaMax < T.nVCs ? nCtaMax : T.nVCs;
     std::vector<int32_t> cnt(C + 1, 0);
@@ -275,7 +277,7 @@ struct Engine {
         int p = ev.spec.priority;
         mask |= (p >= -1 && p < 62) ? (1ull << (p + 1)) : (1ull << 62);
       }
-      if (ev.type != HIVED_EV_SCHEDULE && ev.type != HIVED_EV_DELETE_ALLOCATED) simple = false;
+      if (ev.type != HIVED_EV_SCHEDULE && ev.type != HIVED_EV_DELETE_ALLOCATED) calm = false;
       // the VC that owns the event: a SCHEDULE names it; a DELETE belongs to the VC its group was scheduled under
       // (the event's own VC field is optional, hived.h).  A group id seen under two VCs, or an unknown one: sequential.
       int evVc = ev.spec.vc;
@@ -284,7 +286,7 @@ struct Engine {
         if (g >= 0 && g < (int)groupVcHost.size() && ev.spec.vc >= 0 && ev.spec.vc < T.nVCs) {
           // a group id that THIS batch has already used under another VC (ids are recycled, hived.h "Id lifetime": the
           // old incarnation's release and the new one's creation would meet in the same table row on two CTAs)
-          if (groupStamp[g] == batchStamp && groupVcHost[g] >= 0 && groupVcHost[g] != ev.spec.vc) simple = false;
+          if (groupStamp[g] == batchStamp && groupVcHost[g] >= 0 && groupVcHost[g] != ev.spec.vc) calm = false;
           groupVcHost[g] = ev.spec.vc;
           groupStamp[g] = batchStamp;
         }
@@ -293,9 +295,9 @@ struct Engine {
         if (evVc < 0) evVc = (ev.spec.vc >= 0 && ev.spec.vc < T.nVCs) ? ev.spec.vc : 0;  // unknown group: a no-op wherever it runs
         if (g >= 0 && g < (int)groupStamp.size()) groupStamp[g] = batchStamp;
       }
-      if (evVc < 0 || evVc >= T.nVCs) simple = false;
+      if (evVc < 0 || evVc >= T.nVCs) calm = false;
       if (ev.type == Core::EV_ADD_ALLOCATED) everRecovered = true;
-      if (simple) {
+      if (split && calm) {
         int o = evVc % C;
         ownerOf[i] = (uint8_t)o;
         cnt[o + 1]++;
@@ -308,7 +310,12 @@ struct Engine {
       }
     }
     prioMaskHost = mask;
-    if ((mask & (mask - 1)) != 0 || (mask & 1)) simple = false;  // more than one priority, or opportunistic (-1)
+    if ((mask & (mask - 1)) != 0 || (mask & 1)) calm = false;  // more than one priority, or opportunistic (-1)
+    const bool simple = split && calm;
+    // a calm batch runs the calm leader loop (hived_calm.inc) at any CTA count; HIVED_NO_CALM=1: never (A/B runs)
+    const char* noCalm = getenv("HIVED_NO_CALM");
+    if (noCalm && *noCalm && *noCalm != '0') calm = false;
+    dev.calm = calm ? 1 : 0;
     ownOff.assign(2, 0); ownOff[1] = n;
     poolBase.assign(2, 0); poolBase[1] = poolCap;
     if (simple) {

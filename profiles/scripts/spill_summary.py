@@ -6,9 +6,9 @@ usage: python profiles/scripts/spill_summary.py [path/to/libhived_cuda.so] [--to
 Builds nothing and needs no GPU: extracts the cubin (`cuobjdump -xelf`), disassembles it with line information
 (`nvdisasm -g`) and prints, per kernel, the register count and stack frame (`cuobjdump -res-usage`), its static LDL /
 STL count, and the same count split by out-of-line (ABI-called) function, by the function of hived_core.h /
-hived_lean.inc / hived_runahead.inc whose line range holds the instruction's source line (other files: by file), and
-by source line.  `ptxas -v`'s register line cannot show what setmaxnreg does (it prints the launch-time count), this
-can.  Counts are static instructions, not executions."""
+hived_lean.inc / hived_runahead.inc / hived_calm.inc whose line range holds the instruction's source line (other files:
+by file), and by source line.  `ptxas -v`'s register line cannot show what setmaxnreg does (it prints the launch-time
+count), this can.  Counts are static instructions, not executions."""
 import argparse
 import collections
 import glob
@@ -19,7 +19,7 @@ import tempfile
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 CSRC = os.path.join(ROOT, "hivedscheduler_b200", "csrc")
-FOLDED = ("hived_core.h", "hived_lean.inc", "hived_runahead.inc")
+FOLDED = ("hived_core.h", "hived_lean.inc", "hived_runahead.inc", "hived_calm.inc")
 # a member function's definition in struct Core (two spaces of indentation), template line or not
 DEF = re.compile(r"^  (?:template\s*<.*>\s*)?HIVED_DEV(?:_NOINLINE)?\s+(?:static\s+)?[\w:<>,*&\s]*?\b(\w+)\s*\(")
 
