@@ -71,10 +71,9 @@ struct Sm {
   int part[MAX_WARPS + 32];
   // ---- the current event, fetched with one coalesced 128-byte load
   alignas(16) int32_t ev_words[2][sizeof(hived_event_t) / 4];  // double buffer: the next event arrives while this one runs
-  // ---- lean-lane workspace of the leader warp: values per tree level (lane = level) and per bucket
-  int lw_va[MAXL], lw_pa[MAXL], lw_vold[MAXL], lw_vpc[MAXL], lw_vc0[MAXL], lw_vn[MAXL], lw_pold[MAXL], lw_pst[MAXL], lw_pvc[MAXL],
-      lw_pc0[MAXL], lw_pn[MAXL], lw_pin[MAXL];
-  int lw_omaxv[MAXL], lw_omaxp[MAXL], lw_oflagv[MAXL], lw_oflagp[MAXL];
+  // ---- lean-lane workspace of the leader warp: planLean1's path per tree level (lane = level) — the ancestor, its
+  // binding and its child range (leanDelete1 keeps its path in registers)
+  int lw_va[MAXL], lw_vpc[MAXL], lw_vc0[MAXL], lw_vn[MAXL];
   int un_p[32], un_c[32], un_ls[32];   // planned units: physical cell, commit-time virtual cell, first bound level above
   int un_pl0[32], un_vl0[32], un_node[32];  // ... their first physical / virtual leaf and the view node they will sit in
   int pl_anc[8][32], pl_bnd[8][32];    // planLeanMulti: path and bindings per (level, unit)
