@@ -57,6 +57,11 @@ constexpr int SERVE_MAX_EVENTS = 8, SERVE_POOL_WINDOW = 16384, SERVE_EV_OFF = 32
 constexpr int SERVE_RES_OFF = SERVE_EV_OFF + SERVE_MAX_EVENTS * 32 + SERVE_SUGG_MAX + SERVE_AUX_MAX;
 constexpr int SERVE_DONE_OFF = SERVE_RES_OFF + SERVE_MAX_EVENTS * 32 + SERVE_POOL_WINDOW;
 constexpr int SERVE_SLOT_WORDS = SERVE_DONE_OFF + 32;
+// the slot's header (written by the host, the sequence number last) and its done area (written by the kernel, the done
+// sequence number after the pool offset; the exited flag when it leaves)
+constexpr int SERVE_SEQ = 0, SERVE_N = 1 /* 0: STOP */, SERVE_SUGG_WORDS = 2, SERVE_AUX_WORDS = 3, SERVE_POOL_CAP = 4;
+constexpr int SERVE_DONE_SEQ = SERVE_DONE_OFF, SERVE_DONE_POOL_LO = SERVE_DONE_OFF + 1, SERVE_DONE_POOL_HI = SERVE_DONE_OFF + 2,
+              SERVE_DONE_LAST_SEQ = SERVE_DONE_OFF + 3, SERVE_DONE_EXITED = SERVE_DONE_OFF + 4;
 
 struct Sm {
   int cmd;  // CMD_*
@@ -168,8 +173,8 @@ struct Core {
   // cluster (every other CTA of every rank is parked), the cluster-wide state being this rank's to write
   int mgMode = 0, mgStart = 0;
   bool mgStop = false;
-  // the host judged the batch calm (Engine::prepare): the leader runs the calm loop (hived_calm.inc).  From the Dev
-  // (host builds) or from the launch's scalar word 2 (CUDA kernels)
+  // the host judged the batch calm (Engine::prepare): the leader runs the calm loop (hived_calm.inc).  From the launch
+  // words (runCta)
   bool calm;
   int curEvent;      // index (in the batch) of the event being processed
   bool sharedHeld;   // this event already holds the right to touch the cluster-wide free-list state
@@ -3489,7 +3494,7 @@ struct Core {
   // writes results + pool words back to mapped host memory; the workers serve view passes as in run().  The kernel
   // leaves by itself after `idleSpins` empty polls (a resident kernel must not outlive the calls it serves: any
   // device-wide synchronisation elsewhere in the process would wait for it) or on a STOP request.
-  // slot layout: see ServeSlot in hived_cuda.cu; all offsets in 32-bit words.
+  // slot layout: SERVE_* above; all offsets in 32-bit words.
   HIVED_DEV void serve(volatile int32_t* slot, int seq0, int idleSpins, hived_result_t* stageRes, uint32_t* dSugg, int32_t* dAux,
                        int nPinnedOrder, int nBad) {
     (void)nPinnedOrder; (void)nBad;
@@ -3507,17 +3512,17 @@ struct Core {
     ST(smp()->bkc_sched, -1);
     while (true) {
       int seq = lastSeq, spins = 0;
-      // header line: [0] seq  [1] n (0 = STOP)  [2] suggWords  [3] auxWords  [4] poolCap
+      // the header line, one word per lane
       int hdr = 0;
       while (true) {
         hdr = lane < 8 ? slot[lane] : 0;
-        seq = hv_shfl(hdr, 0);
+        seq = hv_shfl(hdr, SERVE_SEQ);
         if (seq != lastSeq) break;
         if (++spins > idleSpins) break;
       }
       if (seq == lastSeq) break;  // idle: leave
-      const int n = hv_shfl(hdr, 1), suggWords = hv_shfl(hdr, 2), auxWords = hv_shfl(hdr, 3);
-      pool_cap = hv_shfl(hdr, 4);
+      const int n = hv_shfl(hdr, SERVE_N), suggWords = hv_shfl(hdr, SERVE_SUGG_WORDS), auxWords = hv_shfl(hdr, SERVE_AUX_WORDS);
+      pool_cap = hv_shfl(hdr, SERVE_POOL_CAP);
       lastSeq = seq;
       if (n <= 0) break;  // STOP
       // payload: events at word SERVE_EV_OFF, then the suggested bitmaps, then aux
@@ -3547,18 +3552,63 @@ struct Core {
       volatile int32_t* op = out + SERVE_MAX_EVENTS * (int)(sizeof(hived_result_t) / 4);
       const long long used = poolOff < SERVE_POOL_WINDOW ? poolOff : SERVE_POOL_WINDOW;
       for (int i = lane; i < (int)used; i += HIVED_WARPSZ) op[i] = pool[i];
-      if (lane == 0) { slot[SERVE_DONE_OFF + 1] = (int32_t)poolOff; slot[SERVE_DONE_OFF + 2] = (int32_t)(poolOff >> 32); }
+      if (lane == 0) { slot[SERVE_DONE_POOL_LO] = (int32_t)poolOff; slot[SERVE_DONE_POOL_HI] = (int32_t)(poolOff >> 32); }
       __threadfence_system();
       hv_warp_sync();
-      if (lane == 0) slot[SERVE_DONE_OFF] = seq;
+      if (lane == 0) slot[SERVE_DONE_SEQ] = seq;
       hv_warp_sync();
     }
     ST(smp()->cmd, CMD_EXIT);
     hv_cta_sync();
-    if (lane == 0) { __threadfence_system(); slot[SERVE_DONE_OFF + 3] = lastSeq; slot[SERVE_DONE_OFF + 4] = 1; }  // exited
+    if (lane == 0) { __threadfence_system(); slot[SERVE_DONE_LAST_SEQ] = lastSeq; slot[SERVE_DONE_EXITED] = 1; }
   }
 #endif
 };
+
+// One CTA of an events kernel: its launch words in (CtaWords), the program over its share of the batch, its words out.
+// hived_events_kernel and every host build run it; the joint and concurrent builds' kernels write it out.  `dev` is the expression the build's `d` stands for (CUDA) or the context's Dev (host builds); sm is the
+// CTA's shared block; own / ownOff: the owner-sorted event list and its offsets (VC-parallel and partitioned runs),
+// else nullptr.
+HIVED_DEV void runCta(const Dev& dev, Sm* sm, const hived_event_t* events, int n, hived_result_t* results, const uint32_t* sugg,
+                      const int32_t* aux, const int32_t* initLists, int nPinnedOrder, int nBad, int32_t* pool, CtaWords* words,
+                      const int32_t* own, const int32_t* ownOff, int cta, int nCta) {
+  if (hv_tid() == 0) {
+    sm->cmd = CMD_IDLE;
+    sm->panic = 0;
+    sm->lead_k = -1;
+    sm->pool_off = ctaWords(words, cta).poolOff;
+  }
+  hv_block_sync();
+  CtaWords& w = ctaWords(words, cta);
+  Core core(dev, sm, pool, w.poolEnd, nCta);
+  int nOwn = own ? ownOff[cta + 1] - ownOff[cta] : n;
+  if (const long long mg = w.mg) { core.setMultiGpu(mgModeOf(mg), mgCursorOf(mg)); nOwn = mgLimitOf(mg); }
+  core.calm = w.calm != 0;
+  core.run(events, n, results, sugg, aux, initLists, nPinnedOrder, nBad, own ? own + ownOff[cta] : nullptr, nOwn);
+  hv_block_sync();
+  if (hv_tid() == 0) {
+    w.poolOff = sm->pool_off;
+    w.calm = sm->panic;
+    w.mg = sm->stop_k;
+  }
+}
+
+#if defined(__CUDACC__) && !defined(HIVED_SIMT_EMU) && !defined(HIVED_EMU)
+// The one CTA of a resident per-call kernel (Core::serve)
+HIVED_DEV void serveCta(const Dev& dev, volatile int32_t* slot, int seq0, int idleSpins, hived_result_t* stageRes, uint32_t* dSugg,
+                        int32_t* dAux, int nPinnedOrder, int nBad, int32_t* pool) {
+  Sm& sm = g_hived_sm;
+  if (threadIdx.x == 0) {
+    sm.cmd = CMD_IDLE;
+    sm.panic = 0;
+    sm.lead_k = 0x7fffffff;
+    sm.pool_off = 0;
+  }
+  __syncthreads();
+  Core core(dev, &sm, pool, 0, 1);
+  core.serve(slot, seq0, idleSpins, stageRes, dSugg, dAux, nPinnedOrder, nBad);
+}
+#endif
 
 #ifdef HIVED_DEV_IN_CONSTANT
 #undef d

@@ -23,34 +23,13 @@ namespace hived {
 
 constexpr int NT = 512;  // threads per CTA (16 warps); the kernel needs the full register file of one SM
 
-// scalars: 4 words per CTA — [0] pool offset (in: start of the CTA's slice, out: first unused word),
-// [1] end of the slice, [2] in: the batch is calm (Core::calm), out: initialisation panic code
+// scalars: the launch words of every CTA (CtaWords)
 __global__ void __launch_bounds__(NT, 1)
 hived_events_kernel(const hived_event_t* __restrict__ events, int n, hived_result_t* results,
                     const uint32_t* suggPool, const int32_t* aux, const int32_t* initLists, int nPinnedOrder, int nBad,
                     int32_t* pool, long long* scalars, const int32_t* own, const int32_t* ownOff) {
-  Sm& sm = g_hived_sm;
-  const int cta = blockIdx.x;
-  if (threadIdx.x == 0) {
-    sm.cmd = CMD_IDLE;
-    sm.panic = 0;
-    sm.lead_k = -1;
-    sm.pool_off = scalars[cta * 4 + 0];
-  }
-  __syncthreads();
-  Core core(g_hived_dev, &sm, pool, scalars[cta * 4 + 1], gridDim.x);
-  int nOwn = own ? ownOff[cta + 1] - ownOff[cta] : n;
-  // multi-GPU partition: [start, limit) of this CTA's list and the mode, packed by launchProgram (0: an ordinary run)
-  const long long mg = scalars[cta * 4 + 3];
-  if (mg) { core.setMultiGpu((int)((mg >> 62) & 3), (int)(mg & 0x7fffffff)); nOwn = (int)((mg >> 31) & 0x7fffffff); }
-  core.calm = scalars[cta * 4 + 2] != 0;
-  core.run(events, n, results, suggPool, aux, initLists, nPinnedOrder, nBad, own ? own + ownOff[cta] : nullptr, nOwn);
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    scalars[cta * 4 + 0] = sm.pool_off;
-    scalars[cta * 4 + 2] = sm.panic;
-    scalars[cta * 4 + 3] = sm.stop_k;
-  }
+  runCta(g_hived_dev, &g_hived_sm, events, n, results, suggPool, aux, initLists, nPinnedOrder, nBad, pool, (CtaWords*)scalars, own,
+         ownOff, blockIdx.x, gridDim.x);
 }
 
 __global__ void __launch_bounds__(NT, 1) hived_repair_kernel() {
@@ -63,16 +42,7 @@ __global__ void __launch_bounds__(NT, 1) hived_repair_kernel() {
 __global__ void __launch_bounds__(NT, 1)
 hived_serve_kernel(volatile int32_t* slot, int seq0, int idleSpins, hived_result_t* stageRes,
                    uint32_t* dSugg, int32_t* dAux, int nPinnedOrder, int nBad, int32_t* pool) {
-  Sm& sm = g_hived_sm;
-  if (threadIdx.x == 0) {
-    sm.cmd = CMD_IDLE;
-    sm.panic = 0;
-    sm.lead_k = 0x7fffffff;
-    sm.pool_off = 0;
-  }
-  __syncthreads();
-  Core core(g_hived_dev, &sm, pool, 0, 1);
-  core.serve(slot, seq0, idleSpins, stageRes, dSugg, dAux, nPinnedOrder, nBad);
+  serveCta(g_hived_dev, slot, seq0, idleSpins, stageRes, dSugg, dAux, nPinnedOrder, nBad, pool);
 }
 
 static bool cudaOk(cudaError_t e, std::string& err, const char* what) {
@@ -237,10 +207,10 @@ static void serveLeft(ServeChan& c) {
 static void serveStop(ServeChan& c) {
   if (!c.alive) return;
   volatile int32_t* s = c.slotHost;
-  if (!s[SERVE_DONE_OFF + 4]) {
-    s[1] = 0;  // n = 0: STOP
+  if (!s[SERVE_DONE_EXITED]) {
+    s[SERVE_N] = 0;  // STOP
     __sync_synchronize();
-    s[0] = ++c.seq;
+    s[SERVE_SEQ] = ++c.seq;
   }
   cudaStreamSynchronize(c.stream);
   serveLeft(c);
@@ -405,6 +375,23 @@ static_assert(NT / 32 <= MAX_WARPS, "the shared counters are sized for MAX_WARPS
 
 static int concLaunch(Engine& e, ServeChan& c, int n);
 
+// The end of a launch queued on `st` for the contexts es[0..k) (its words' copy-back queued after t's stop event): wait
+// for it, then every context's kernel time.  HIVED_ERR_PLATFORM with every context's err naming `kernel` if it failed.
+static int launchDone(Engine* const* es, int k, CudaTimers* t, cudaStream_t st, const char* kernel) {
+  cudaError_t err = cudaStreamSynchronize(st);
+  if (err != cudaSuccess || (err = cudaGetLastError()) != cudaSuccess) {
+    for (int y = 0; y < k; y++) es[y]->err = std::string(kernel) + " failed: " + cudaGetErrorString(err);
+    return HIVED_ERR_PLATFORM;
+  }
+  float ms = 0.f;
+  cudaEventElapsedTime(&ms, t->start, t->stop);
+  for (int y = 0; y < k; y++) {
+    es[y]->lastKernelMs = ms;
+    es[y]->kernelMsTotal += ms;
+  }
+  return 0;
+}
+
 int launchProgram(Engine& e, int n, bool withInit) {
   // a concurrent context's batch: its own stream, constant slot and seats, no turn
   if (t_own && e.stream && t_own == ((CudaTimers*)e.stream)->conc && !withInit && !e.mgMode) return concLaunch(e, *t_own, n);
@@ -433,61 +420,38 @@ int launchProgram(Engine& e, int n, bool withInit) {
     e.kernelLaunches++;
     return 0;
   }
-  long long scal[MAX_CTAS * 4] = {0};
-  for (int c = 0; c < C; c++) {
-    scal[c * 4 + 0] = withInit ? 0 : (mgMode ? e.mgPoolCur[c] : e.poolBase[c]);
-    scal[c * 4 + 1] = withInit ? 0 : e.poolBase[c + 1];
-    scal[c * 4 + 2] = !withInit && !mgMode && e.dev.calm;
-    if (mgMode) scal[c * 4 + 3] = ((long long)mgMode << 62) | ((long long)e.mgLimit[c] << 31) | (long long)e.mgCursor[c];
-  }
-  cudaMemcpyAsync(e.dScalars.p, scal, sizeof scal, cudaMemcpyHostToDevice, t->stream);
+  CtaWords w[MAX_CTAS] = {};
+  e.packCtaWords(w, C, withInit);
+  cudaMemcpyAsync(e.dScalars.p, w, sizeof w, cudaMemcpyHostToDevice, t->stream);
   cudaEventRecord(t->start, t->stream);
+  const hived_event_t* events = (const hived_event_t*)e.dEvents.p;
+  hived_result_t* results = (hived_result_t*)e.dResults.p;
+  const uint32_t* sugg = e.hasSugg ? (const uint32_t*)e.dSugg.p : nullptr;
+  const int32_t* aux = e.hasAux ? (const int32_t*)e.dAux.p : nullptr;
+  const int32_t* init = withInit ? (const int32_t*)e.dInit.p : nullptr;
+  int32_t* pool = (int32_t*)e.dPool.p;
+  long long* scalars = (long long*)e.dScalars.p;
   const int32_t* own = (C > 1 || mgMode) ? (const int32_t*)e.dOwn.p : nullptr;
-  if (C > 1 && !mgMode) {
+  const int32_t* ownOff = own ? own + n : nullptr;
+  const bool parallel = C > 1 && !mgMode;
+  if (parallel) {
     // The CTAs of a VC-parallel batch wait for each other (ordered shared sections): launch them cooperatively, so
     // that the runtime guarantees that all of them are resident at the same time.
-    const hived_event_t* aEvents = (const hived_event_t*)e.dEvents.p;
-    int aN = n;
-    hived_result_t* aResults = (hived_result_t*)e.dResults.p;
-    const uint32_t* aSugg = e.hasSugg ? (const uint32_t*)e.dSugg.p : nullptr;
-    const int32_t* aAux = e.hasAux ? (const int32_t*)e.dAux.p : nullptr;
-    const int32_t* aInit = nullptr;
-    int aPinned = e.nPinnedOrder, aBad = e.nBad;
-    int32_t* aPool = (int32_t*)e.dPool.p;
-    long long* aScal = (long long*)e.dScalars.p;
-    const int32_t* aOwn = own;
-    const int32_t* aOwnOff = own + n;
-    void* args[] = {&aEvents, &aN, &aResults, &aSugg, &aAux, &aInit, &aPinned, &aBad, &aPool, &aScal, &aOwn, &aOwnOff};
+    void* args[] = {&events, &n, &results, &sugg, &aux, &init, &e.nPinnedOrder, &e.nBad, &pool, &scalars, &own, &ownOff};
     cudaError_t le = cudaLaunchCooperativeKernel((const void*)hived_events_kernel, dim3(C), dim3(NT), args, 0, t->stream);
     if (le != cudaSuccess) {
       e.err = std::string("cooperative launch of hived_events_kernel failed: ") + cudaGetErrorString(le);
       return HIVED_ERR_PLATFORM;
     }
+    hived_repair_kernel<<<1, NT, 0, t->stream>>>();
   } else {
-    hived_events_kernel<<<C, NT, 0, t->stream>>>(
-        (const hived_event_t*)e.dEvents.p, n, (hived_result_t*)e.dResults.p,
-        e.hasSugg ? (const uint32_t*)e.dSugg.p : nullptr, e.hasAux ? (const int32_t*)e.dAux.p : nullptr,
-        withInit ? (const int32_t*)e.dInit.p : nullptr, e.nPinnedOrder, e.nBad, (int32_t*)e.dPool.p, (long long*)e.dScalars.p, own,
-        own ? own + n : nullptr);
+    hived_events_kernel<<<C, NT, 0, t->stream>>>(events, n, results, sugg, aux, init, e.nPinnedOrder, e.nBad, pool, scalars, own, ownOff);
   }
-  if (C > 1 && !mgMode) hived_repair_kernel<<<1, NT, 0, t->stream>>>();
   cudaEventRecord(t->stop, t->stream);
-  cudaMemcpyAsync(scal, e.dScalars.p, sizeof scal, cudaMemcpyDeviceToHost, t->stream);
-  cudaError_t err = cudaStreamSynchronize(t->stream);
-  if (err != cudaSuccess || (err = cudaGetLastError()) != cudaSuccess) {
-    e.err = std::string("hived_events_kernel failed: ") + cudaGetErrorString(err);
-    return HIVED_ERR_PLATFORM;
-  }
-  float ms = 0.f;
-  cudaEventElapsedTime(&ms, t->start, t->stop);
-  e.lastKernelMs = ms;
-  e.kernelMsTotal += ms;
-  e.kernelLaunches += (C > 1 && !mgMode) ? 2 : 1;
-  e.poolEnd.assign(C, 0);
-  for (int c = 0; c < C; c++) e.poolEnd[c] = scal[c * 4 + 0];
-  if (mgMode) { e.mgStopOut.assign(C, 0); for (int c = 0; c < C; c++) e.mgStopOut[c] = (int32_t)scal[c * 4 + 3]; }
-  e.poolOff = scal[0];
-  if (withInit && scal[2]) { e.err = "initialisation panicked on the device"; return (int)scal[2]; }
+  cudaMemcpyAsync(w, e.dScalars.p, sizeof w, cudaMemcpyDeviceToHost, t->stream);
+  Engine* es[] = {&e};
+  if (int rc = launchDone(es, 1, t, t->stream, "hived_events_kernel")) return rc;
+  if (int rc = e.takeCtaWords(w, C, withInit, parallel ? 2 : 1)) { e.err = "initialisation panicked on the device"; return rc; }
   return 0;
 }
 
@@ -498,14 +462,14 @@ static int concLaunch(Engine& e, ServeChan& c, int n) {
   CudaTimers* t = (CudaTimers*)e.stream;
   if (int rc = takeCopyError(e.err)) return rc;  // a staging copy of this batch failed
   const int C = e.launchCta;
-  long long scal[MAX_CTAS * 4] = {0};
-  for (int k = 0; k < C; k++) { scal[k * 4 + 0] = e.poolBase[k]; scal[k * 4 + 1] = e.poolBase[k + 1]; scal[k * 4 + 2] = e.dev.calm; }
+  CtaWords w[MAX_CTAS] = {};
+  e.packCtaWords(w, C, false);
   const ManySlot q{(const hived_event_t*)e.dEvents.p, (hived_result_t*)e.dResults.p,
-                   e.hasSugg ? (const uint32_t*)e.dSugg.p : nullptr, (int32_t*)e.dPool.p, (long long*)e.dScalars.p,
+                   e.hasSugg ? (const uint32_t*)e.dSugg.p : nullptr, (int32_t*)e.dPool.p, (CtaWords*)e.dScalars.p,
                    C > 1 ? (const int32_t*)e.dOwn.p : nullptr, n, C, e.nPinnedOrder, e.nBad};
   SeatHold seats(seatsOf(e), C);
   if (!seats.ok()) return seatError(e, C);
-  cudaMemcpyAsync(e.dScalars.p, scal, sizeof scal, cudaMemcpyHostToDevice, c.stream);
+  cudaMemcpyAsync(e.dScalars.p, w, sizeof w, cudaMemcpyHostToDevice, c.stream);
   cudaEventRecord(t->start, c.stream);
   cudaError_t err = concBatchLaunch(c.conc, q, c.stream);
   if (err != cudaSuccess) {
@@ -515,20 +479,10 @@ static int concLaunch(Engine& e, ServeChan& c, int n) {
     return HIVED_ERR_PLATFORM;
   }
   cudaEventRecord(t->stop, c.stream);
-  cudaMemcpyAsync(scal, e.dScalars.p, sizeof scal, cudaMemcpyDeviceToHost, c.stream);
-  err = cudaStreamSynchronize(c.stream);
-  if (err != cudaSuccess || (err = cudaGetLastError()) != cudaSuccess) {
-    e.err = std::string("hived_events_conc_kernel failed: ") + cudaGetErrorString(err);
-    return HIVED_ERR_PLATFORM;
-  }
-  float ms = 0.f;
-  cudaEventElapsedTime(&ms, t->start, t->stop);
-  e.lastKernelMs = ms;
-  e.kernelMsTotal += ms;
-  e.kernelLaunches += C > 1 ? 2 : 1;
-  e.poolEnd.assign(C, 0);
-  for (int k = 0; k < C; k++) e.poolEnd[k] = scal[k * 4 + 0];
-  e.poolOff = scal[0];
+  cudaMemcpyAsync(w, e.dScalars.p, sizeof w, cudaMemcpyDeviceToHost, c.stream);
+  Engine* es[] = {&e};
+  if (int rc = launchDone(es, 1, t, c.stream, "hived_events_conc_kernel")) return rc;
+  e.takeCtaWords(w, C, false, C > 1 ? 2 : 1);
   return 0;
 }
 
@@ -563,17 +517,17 @@ int bk_launch_many(Engine* const* es, int k) {
   const int fit = manyCoResident(e0.deviceOrdinal) - concInUse(dv);
   if (fit <= 0) return fail("joint launch: cannot query the co-resident CTA limit");
   CudaTimers* t = (CudaTimers*)e0.stream;
-  std::vector<long long> scal((size_t)k * MAX_CTAS * 4, 0);
+  std::vector<CtaWords> words((size_t)k * MAX_CTAS);
   ManyArgs a;
   const Dev* devs[HIVED_MANY_MAX];
   for (int y = 0; y < k; y++) {
     Engine& e = *es[y];
     const int C = e.launchCta;
-    long long* s = &scal[(size_t)y * MAX_CTAS * 4];
-    for (int c = 0; c < C; c++) { s[c * 4 + 0] = e.poolBase[c]; s[c * 4 + 1] = e.poolBase[c + 1]; s[c * 4 + 2] = e.dev.calm; }
-    cudaMemcpyAsync(e.dScalars.p, s, MAX_CTAS * 4 * sizeof(long long), cudaMemcpyHostToDevice, t->stream);
+    CtaWords* w = &words[(size_t)y * MAX_CTAS];
+    e.packCtaWords(w, C, false);
+    cudaMemcpyAsync(e.dScalars.p, w, MAX_CTAS * sizeof(CtaWords), cudaMemcpyHostToDevice, t->stream);
     a.slot[y] = ManySlot{(const hived_event_t*)e.dEvents.p, (hived_result_t*)e.dResults.p,
-                         e.hasSugg ? (const uint32_t*)e.dSugg.p : nullptr, (int32_t*)e.dPool.p, (long long*)e.dScalars.p,
+                         e.hasSugg ? (const uint32_t*)e.dSugg.p : nullptr, (int32_t*)e.dPool.p, (CtaWords*)e.dScalars.p,
                          C > 1 ? (const int32_t*)e.dOwn.p : nullptr, e.stagedN, C, e.nPinnedOrder, e.nBad};
     devs[y] = &e.dev;
   }
@@ -604,22 +558,9 @@ int bk_launch_many(Engine* const* es, int k) {
   }
   cudaEventRecord(t->stop, t->stream);
   for (int y = 0; y < k; y++)
-    cudaMemcpyAsync(&scal[(size_t)y * MAX_CTAS * 4], es[y]->dScalars.p, MAX_CTAS * 4 * sizeof(long long), cudaMemcpyDeviceToHost, t->stream);
-  cudaError_t ce = cudaStreamSynchronize(t->stream);
-  if (ce != cudaSuccess || (ce = cudaGetLastError()) != cudaSuccess) return fail(std::string("hived_events_many_kernel failed: ") + cudaGetErrorString(ce));
-  float ms = 0.f;
-  cudaEventElapsedTime(&ms, t->start, t->stop);
-  for (int y = 0; y < k; y++) {
-    Engine& e = *es[y];
-    const int C = e.launchCta;
-    const long long* s = &scal[(size_t)y * MAX_CTAS * 4];
-    e.lastKernelMs = ms;
-    e.kernelMsTotal += ms;
-    e.kernelLaunches += C > 1 ? 2 : 1;
-    e.poolEnd.assign(C, 0);
-    for (int c = 0; c < C; c++) e.poolEnd[c] = s[c * 4 + 0];
-    e.poolOff = s[0];
-  }
+    cudaMemcpyAsync(&words[(size_t)y * MAX_CTAS], es[y]->dScalars.p, MAX_CTAS * sizeof(CtaWords), cudaMemcpyDeviceToHost, t->stream);
+  if (int rc = launchDone(es, k, t, t->stream, "hived_events_many_kernel")) return rc;
+  for (int y = 0; y < k; y++) es[y]->takeCtaWords(&words[(size_t)y * MAX_CTAS], es[y]->launchCta, false, es[y]->launchCta > 1 ? 2 : 1);
   return 0;
 }
 
@@ -667,12 +608,15 @@ static int serveCall(Engine& e, ServeChan& c, const hived_event_t* events, int n
   int32_t* hs = pay + SERVE_MAX_EVENTS * (int)(sizeof(hived_event_t) / 4);
   if (hasSugg) memcpy(hs, suggPool, (size_t)suggWords * 4);
   if (hasAux) memcpy(hs + (hasSugg ? suggWords : 0), aux, (size_t)auxWords * 4);
-  s[1] = n; s[2] = hasSugg ? (int32_t)suggWords : 0; s[3] = hasAux ? (int32_t)auxWords : 0; s[4] = (int32_t)cap;
+  s[SERVE_N] = n;
+  s[SERVE_SUGG_WORDS] = hasSugg ? (int32_t)suggWords : 0;
+  s[SERVE_AUX_WORDS] = hasAux ? (int32_t)auxWords : 0;
+  s[SERVE_POOL_CAP] = (int32_t)cap;
   const int seq = ++c.seq;
   __sync_synchronize();
-  s[0] = seq;
+  s[SERVE_SEQ] = seq;
   auto launch = [&]() {
-    s[SERVE_DONE_OFF + 4] = 0;
+    s[SERVE_DONE_EXITED] = 0;
     __sync_synchronize();
     // 1500 polls over PCIe: the kernel leaves after 1.5-2 ms without a request on an H100
     // (profiles/micro/resident_idle_timeout.py)
@@ -696,11 +640,11 @@ static int serveCall(Engine& e, ServeChan& c, const hived_event_t* events, int n
   if (!c.alive && !launch()) { serveLeft(c); return HIVED_ERR_PLATFORM; }
   // wait for `done`; a kernel that left just before the request arrived is replaced
   long long spins = 0;
-  while (s[SERVE_DONE_OFF] != seq) {
-    if (s[SERVE_DONE_OFF + 4] && s[SERVE_DONE_OFF] != seq) {
+  while (s[SERVE_DONE_SEQ] != seq) {
+    if (s[SERVE_DONE_EXITED] && s[SERVE_DONE_SEQ] != seq) {
       cudaError_t err = cudaStreamSynchronize(c.stream);
       if (err != cudaSuccess) { e.err = std::string("hived_serve_kernel failed: ") + cudaGetErrorString(err); serveLeft(c); return HIVED_ERR_PLATFORM; }
-      if (s[SERVE_DONE_OFF] == seq) break;
+      if (s[SERVE_DONE_SEQ] == seq) break;
       if (!launch()) { serveLeft(c); return HIVED_ERR_PLATFORM; }
     }
     if ((++spins & 0xfffff) == 0) {  // every ~million polls: is the kernel still healthy?
@@ -717,7 +661,7 @@ static int serveCall(Engine& e, ServeChan& c, const hived_event_t* events, int n
   }
   __sync_synchronize();
   c.served++;
-  const long long used = (long long)(uint32_t)s[SERVE_DONE_OFF + 1] | ((long long)s[SERVE_DONE_OFF + 2] << 32);
+  const long long used = (long long)(uint32_t)s[SERVE_DONE_POOL_LO] | ((long long)s[SERVE_DONE_POOL_HI] << 32);
   e.poolOff = used;
   e.poolEnd.assign(1, used);
   e.lastKernelMs = 0.f;
@@ -760,7 +704,7 @@ int bk_run_small(Engine& e, const hived_event_t* events, int n, const uint32_t* 
   static thread_local SmallStage stage;  // per host thread; the shim serialises calls per context anyway
   const bool hasSugg = suggPool != nullptr && suggWords > 0;
   const int64_t window = poolCap < SMALL_POOL_WINDOW ? poolCap : SMALL_POOL_WINDOW;
-  const size_t oEv = 0, oScal = oEv + (size_t)n * sizeof(hived_event_t), oSugg = oScal + 4 * sizeof(long long),
+  const size_t oEv = 0, oScal = oEv + (size_t)n * sizeof(hived_event_t), oSugg = oScal + sizeof(CtaWords),
                oAux = oSugg + (hasSugg ? (size_t)suggWords * 4 : 0), oRes = (oAux + (hasAux ? (size_t)auxWords * 4 : 0) + 15) & ~(size_t)15,
                oPool = oRes + (size_t)n * sizeof(hived_result_t), total = oPool + (size_t)(window > 0 ? window : 1) * 4;
   if (total > stage.bytes) {
@@ -784,13 +728,14 @@ int bk_run_small(Engine& e, const hived_event_t* events, int n, const uint32_t* 
   e.poolCapWords = poolCap; e.stagedN = n; e.stagedEvents = events; e.canonicalDone = false;
   char* h = stage.host;
   memcpy(h + oEv, events, (size_t)n * sizeof(hived_event_t));
-  long long* scal = (long long*)(h + oScal);
-  scal[0] = 0; scal[1] = poolCap; scal[2] = 0; scal[3] = 0;
+  CtaWords* w = (CtaWords*)(h + oScal);
+  e.packCtaWords(w, 1, false);
+  w->calm = 0;  // (prepare() did not judge these events: they take the general loop)
   if (hasSugg) memcpy(h + oSugg, suggPool, (size_t)suggWords * 4);
   if (hasAux) memcpy(h + oAux, aux, (size_t)auxWords * 4);
   cudaStream_t st = t->stream;
   cudaMemcpyAsync(e.dEvents.p, h + oEv, (size_t)n * sizeof(hived_event_t), cudaMemcpyHostToDevice, st);
-  cudaMemcpyAsync(e.dScalars.p, scal, 4 * sizeof(long long), cudaMemcpyHostToDevice, st);
+  cudaMemcpyAsync(e.dScalars.p, w, sizeof(CtaWords), cudaMemcpyHostToDevice, st);
   if (hasSugg) cudaMemcpyAsync(e.dSugg.p, h + oSugg, (size_t)suggWords * 4, cudaMemcpyHostToDevice, st);
   if (hasAux) cudaMemcpyAsync(e.dAux.p, h + oAux, (size_t)auxWords * 4, cudaMemcpyHostToDevice, st);
   cudaEventRecord(t->start, st);
@@ -798,21 +743,12 @@ int bk_run_small(Engine& e, const hived_event_t* events, int n, const uint32_t* 
                                         hasSugg ? (const uint32_t*)e.dSugg.p : nullptr, hasAux ? (const int32_t*)e.dAux.p : nullptr,
                                         nullptr, e.nPinnedOrder, e.nBad, (int32_t*)e.dPool.p, (long long*)e.dScalars.p, nullptr, nullptr);
   cudaEventRecord(t->stop, st);
-  cudaMemcpyAsync(scal, e.dScalars.p, 4 * sizeof(long long), cudaMemcpyDeviceToHost, st);
+  cudaMemcpyAsync(w, e.dScalars.p, sizeof(CtaWords), cudaMemcpyDeviceToHost, st);
   cudaMemcpyAsync(h + oRes, e.dResults.p, (size_t)n * sizeof(hived_result_t), cudaMemcpyDeviceToHost, st);
   if (window > 0) cudaMemcpyAsync(h + oPool, e.dPool.p, (size_t)window * 4, cudaMemcpyDeviceToHost, st);
-  cudaError_t err = cudaStreamSynchronize(st);
-  if (err != cudaSuccess || (err = cudaGetLastError()) != cudaSuccess) {
-    e.err = std::string("hived_events_kernel failed: ") + cudaGetErrorString(err);
-    return HIVED_ERR_PLATFORM;
-  }
-  float ms = 0.f;
-  cudaEventElapsedTime(&ms, t->start, t->stop);
-  e.lastKernelMs = ms;
-  e.kernelMsTotal += ms;
-  e.kernelLaunches += 1;
-  e.poolOff = scal[0];
-  e.poolEnd.assign(1, scal[0]);
+  Engine* es[] = {&e};
+  if (int rc = launchDone(es, 1, t, st, "hived_events_kernel")) return rc;
+  e.takeCtaWords(w, 1, false, 1);
   if (e.poolOff > poolCap) return HIVED_ERR_CAPACITY;
   memcpy(res, h + oRes, (size_t)n * sizeof(hived_result_t));
   const int64_t got = e.poolOff < window ? e.poolOff : window;

@@ -15,25 +15,26 @@ constexpr int NT = 512;  // as hived_cuda.cu: 16 warps, the whole register file 
 
 // one batch of the context: CTA x of its C CTAs (grid (C, 1)), arguments as for hived_events_kernel
 __global__ void __launch_bounds__(NT, 1) hived_events_conc_kernel(const __grid_constant__ ManySlot q) {
+  // (runCta's body, written out as in hived_events_many_kernel, for the same reason)
   Sm& sm = g_hived_sm;
   const int cta = blockIdx.x;
   if (threadIdx.x == 0) {
     sm.cmd = CMD_IDLE;
     sm.panic = 0;
     sm.lead_k = -1;
-    sm.pool_off = q.scalars[cta * 4 + 0];
+    sm.pool_off = ctaWords(q.words, cta).poolOff;
   }
   __syncthreads();
-  Core core(g_hived_devs[hv_slot_base()], &sm, q.pool, q.scalars[cta * 4 + 1], q.C);
+  Core core(g_hived_devs[hv_slot_base()], &sm, q.pool, ctaWords(q.words, cta).poolEnd, q.C);
   const int32_t* ownOff = q.own ? q.own + q.n : nullptr;
   const int nOwn = q.own ? ownOff[cta + 1] - ownOff[cta] : q.n;
-  core.calm = q.scalars[cta * 4 + 2] != 0;
+  core.calm = ctaWords(q.words, cta).calm != 0;
   core.run(q.events, q.n, q.results, q.sugg, nullptr, nullptr, q.nPinnedOrder, q.nBad, q.own ? q.own + ownOff[cta] : nullptr, nOwn);
   __syncthreads();
   if (threadIdx.x == 0) {
-    q.scalars[cta * 4 + 0] = sm.pool_off;
-    q.scalars[cta * 4 + 2] = sm.panic;
-    q.scalars[cta * 4 + 3] = sm.stop_k;
+    ctaWords(q.words, cta).poolOff = sm.pool_off;
+    ctaWords(q.words, cta).calm = sm.panic;
+    ctaWords(q.words, cta).mg = sm.stop_k;
   }
 }
 
@@ -47,16 +48,7 @@ __global__ void __launch_bounds__(NT, 1) hived_repair_conc_kernel() {
 __global__ void __launch_bounds__(NT, 1)
 hived_serve_conc_kernel(volatile int32_t* slot, int seq0, int idleSpins, hived_result_t* stageRes, uint32_t* dSugg,
                         int32_t* dAux, int nPinnedOrder, int nBad, int32_t* pool) {
-  Sm& sm = g_hived_sm;
-  if (threadIdx.x == 0) {
-    sm.cmd = CMD_IDLE;
-    sm.panic = 0;
-    sm.lead_k = 0x7fffffff;
-    sm.pool_off = 0;
-  }
-  __syncthreads();
-  Core core(g_hived_devs[hv_slot_base()], &sm, pool, 0, 1);
-  core.serve(slot, seq0, idleSpins, stageRes, dSugg, dAux, nPinnedOrder, nBad);
+  serveCta(g_hived_devs[hv_slot_base()], slot, seq0, idleSpins, stageRes, dSugg, dAux, nPinnedOrder, nBad, pool);
 }
 
 }  // namespace conc

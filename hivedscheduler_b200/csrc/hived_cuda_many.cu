@@ -16,24 +16,26 @@ __global__ void __launch_bounds__(NT, 1) hived_events_many_kernel(const __grid_c
   const ManySlot& q = a.slot[blockIdx.y];
   const int cta = blockIdx.x;
   if (cta >= q.C) return;
+  // (runCta's body, written out: its arguments would be read from the parameter space at the call, before the barrier,
+  // and change this kernel's code)
   Sm& sm = g_hived_sm;
   if (threadIdx.x == 0) {
     sm.cmd = CMD_IDLE;
     sm.panic = 0;
     sm.lead_k = -1;
-    sm.pool_off = q.scalars[cta * 4 + 0];
+    sm.pool_off = ctaWords(q.words, cta).poolOff;
   }
   __syncthreads();
-  Core core(g_hived_devs[blockIdx.y], &sm, q.pool, q.scalars[cta * 4 + 1], q.C);
+  Core core(g_hived_devs[blockIdx.y], &sm, q.pool, ctaWords(q.words, cta).poolEnd, q.C);
   const int32_t* ownOff = q.own ? q.own + q.n : nullptr;
   const int nOwn = q.own ? ownOff[cta + 1] - ownOff[cta] : q.n;
-  core.calm = q.scalars[cta * 4 + 2] != 0;
+  core.calm = ctaWords(q.words, cta).calm != 0;
   core.run(q.events, q.n, q.results, q.sugg, nullptr, nullptr, q.nPinnedOrder, q.nBad, q.own ? q.own + ownOff[cta] : nullptr, nOwn);
   __syncthreads();
   if (threadIdx.x == 0) {
-    q.scalars[cta * 4 + 0] = sm.pool_off;
-    q.scalars[cta * 4 + 2] = sm.panic;
-    q.scalars[cta * 4 + 3] = sm.stop_k;
+    ctaWords(q.words, cta).poolOff = sm.pool_off;
+    ctaWords(q.words, cta).calm = sm.panic;
+    ctaWords(q.words, cta).mg = sm.stop_k;
   }
 }
 

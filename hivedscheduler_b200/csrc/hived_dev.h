@@ -118,8 +118,8 @@ struct Dev {
   int32_t* epoch;          // [MAX_CTAS] per-CTA stamp for vx_stamp
   const Scratch* scratch;  // [nCta] private scratch arrays of every CTA
   int32_t* progress;       // [MAX_CTAS] index of the event each CTA is working on (multi-CTA ordering)
-  // the staged batch runs the calm leader loop (Engine::prepare, hived_calm.inc).  Read from here by the host builds;
-  // the CUDA kernels, whose Dev is a copy in the constant bank, get it in the launch's scalar word 2
+  // the staged batch runs the calm leader loop (Engine::prepare, hived_calm.inc).  The host passes it to every build's
+  // CTAs in CtaWords::calm: the CUDA kernels' Dev is a copy in the constant bank, loaded when the context changes
   int32_t calm;
 };
 
@@ -141,6 +141,31 @@ enum {
 };
 
 constexpr int MAX_CTAS = 32;
+
+// The launch words of one CTA of an events kernel: the host fills them (Engine::packCtaWords), the CTA body (runCta,
+// hived_core.h) reads them at its start and writes its results back into them at its end, and the host takes those
+// (Engine::takeCtaWords).  A launch's record (Engine::dScalars) holds MAX_CTAS of them, CTA c's at index c.
+struct CtaWords {
+  long long poolOff;  // in: start of the CTA's pool slice; out: the first word of the slice the CTA did not use
+  long long poolEnd;  // in: end of the slice
+  long long calm;     // in: the batch runs the calm leader loop (Dev::calm); out: the initialisation's panic code
+  long long mg;       // in: the multi-GPU partition's mode, limit and cursor (packMg), 0 in an ordinary run;
+                      // out: Sm::stop_k, where the CTA stopped in its event list
+};
+static_assert(sizeof(CtaWords) == 32, "four 8-byte words per CTA");
+// CTA c's words in a launch's record.  Addressed as the record's 8-byte words, four per CTA: the kernels' code depends
+// on the index being formed in 32 bits, as it always was.
+HIVED_HD CtaWords& ctaWords(CtaWords* record, int c) {
+  return *reinterpret_cast<CtaWords*>(reinterpret_cast<long long*>(record) + c * 4);
+}
+// CtaWords::mg: mode in bits 62-63, limit (the end of the CTA's run in its event list) in bits 31-61, cursor (its start)
+// in bits 0-30
+HIVED_HD long long packMg(int mode, int limit, int cursor) {
+  return ((long long)mode << 62) | ((long long)limit << 31) | (long long)cursor;
+}
+HIVED_HD int mgModeOf(long long w) { return (int)((w >> 62) & 3); }
+HIVED_HD int mgLimitOf(long long w) { return (int)((w >> 31) & 0x7fffffff); }
+HIVED_HD int mgCursorOf(long long w) { return (int)(w & 0x7fffffff); }
 
 // group flags
 enum { GF_LAZY_ENABLE = 1, GF_HAS_VIRTUAL = 2, GF_LAZY_PREEMPTED = 4 };

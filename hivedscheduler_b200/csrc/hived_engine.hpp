@@ -237,7 +237,7 @@ struct Engine {
     nBad = (int)T.bad_init_order.size();
     dInit.ensure((init.size() + 1) * 4);
     if (!init.empty()) bk_h2d(dInit.p, init.data(), init.size() * 4);
-    dScalars.ensure(MAX_CTAS * 4 * sizeof(long long));
+    dScalars.ensure(MAX_CTAS * sizeof(CtaWords));
     dOwn.ensure(64);
     dPool.ensure(4096 * 4);
     dResults.ensure(sizeof(hived_result_t));
@@ -481,6 +481,29 @@ struct Engine {
       for (int c = 0; c < launchCta; c++) if (ownOff[c + 1] > ownOff[c]) prog[c] = own[ownOff[c]];
       bk_h2d(dev.progress, prog.data(), MAX_CTAS * 4);
     }
+  }
+  // The launch words of the next run's C CTAs (hived_dev.h CtaWords; the initialisation runs one CTA without a pool)
+  void packCtaWords(CtaWords* w, int C, bool withInit) const {
+    const int mode = withInit ? 0 : mgMode;
+    for (int c = 0; c < C; c++) {
+      w[c].poolOff = withInit ? 0 : (mode ? mgPoolCur[c] : poolBase[c]);
+      w[c].poolEnd = withInit ? 0 : poolBase[c + 1];
+      w[c].calm = !withInit && !mode && dev.calm;
+      w[c].mg = mode ? packMg(mode, mgLimit[c], mgCursor[c]) : 0;
+    }
+  }
+  // ... and what the run left in them, after `launches` kernels; the initialisation's panic code (the caller says
+  // why), else 0
+  int takeCtaWords(const CtaWords* w, int C, bool withInit, int launches) {
+    kernelLaunches += launches;
+    poolEnd.assign(C, 0);
+    for (int c = 0; c < C; c++) poolEnd[c] = w[c].poolOff;
+    if (mgMode && !withInit) {
+      mgStopOut.assign(C, 0);
+      for (int c = 0; c < C; c++) mgStopOut[c] = (int32_t)w[c].mg;
+    }
+    poolOff = w[0].poolOff;
+    return withInit ? (int)w[0].calm : 0;
   }
 
   // ---- multi-GPU partition of one calm batch (include/hived_multigpu.h) --------------------------------------

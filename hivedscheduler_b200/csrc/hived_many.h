@@ -16,7 +16,7 @@ struct ManySlot {
   hived_result_t* results;
   const uint32_t* sugg;     // nullptr: no suggested-node pool
   int32_t* pool;
-  long long* scalars;       // 4 words per CTA, as for hived_events_kernel
+  CtaWords* words;          // the launch words of every CTA, as for hived_events_kernel
   const int32_t* own;       // VC-parallel run: owner-sorted event list, then the C + 1 list offsets; else nullptr
   int n, C, nPinnedOrder, nBad;
 };

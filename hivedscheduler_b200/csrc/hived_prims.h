@@ -29,6 +29,7 @@ inline void hv_regs_other_group() {}
 inline void hv_nanosleep() {}
 inline void hv_touch(const void*) {}
 inline void hv_cta_sync() {}
+inline void hv_block_sync() {}
 inline void hv_publish_smem(int* p, int v) { *(volatile int*)p = v; }
 inline int hv_peek_smem(int* p) { return *(volatile int*)p; }
 inline void hv_warp_sync() {}
@@ -100,6 +101,7 @@ inline void hv_regs_other_group() {}
 inline void hv_nanosleep() { simt::yield_to_scheduler(); }
 inline void hv_touch(const void* p) { (void)*(const volatile char*)p; }
 inline void hv_cta_sync() { simt::cta_barrier_n(hv_nth()); }
+inline void hv_block_sync() { simt::cta_barrier(); }
 inline void hv_publish_smem(int* p, int v) { *(volatile int*)p = v; }
 inline int hv_peek_smem(int* p) { simt::yield_to_scheduler(); return *(volatile int*)p; }
 inline void hv_warp_sync() { simt::warp_collective(0, [](const int*, int*) {}); }
@@ -205,6 +207,8 @@ __device__ __forceinline__ void hv_cta_sync() { asm volatile("bar.sync 1, %0;" :
 #else
 __device__ __forceinline__ void hv_cta_sync() { asm volatile("barrier.sync 1, %0;" ::"r"(blockDim.x - 32) : "memory"); }
 #endif
+// every thread of the CTA, the run-ahead warp included (the entry and exit of a kernel's CTA body)
+__device__ __forceinline__ void hv_block_sync() { __syncthreads(); }
 // a progress word in SHARED memory polled by another warp of the CTA (the run-ahead warp follows the leader): atomic
 // on both sides, so that the intended concurrent access is not a data race (compute-sanitizer racecheck)
 #ifdef HIVED_AB_VOLATILE_PUBLISH  // (A/B builds only)

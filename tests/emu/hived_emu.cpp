@@ -31,16 +31,12 @@ int launchProgram(Engine& e, int n, bool withInit) {
   e.poolBase[1] = withInit ? 0 : e.poolCapWords;
   static Sm sm;
   memset(&sm, 0, sizeof sm);
-  sm.pool_off = 0;
-  sm.lead_k = -1;
-  Core core(e.dev, &sm, (int32_t*)e.dPool.p, withInit ? 0 : e.poolCapWords, 1);
-  core.run((const hived_event_t*)e.dEvents.p, n, (hived_result_t*)e.dResults.p,
-           e.hasSugg ? (const uint32_t*)e.dSugg.p : nullptr, e.hasAux ? (const int32_t*)e.dAux.p : nullptr,
-           withInit ? (const int32_t*)e.dInit.p : nullptr, e.nPinnedOrder, e.nBad, nullptr, n);
-  e.poolOff = sm.pool_off;
-  e.poolEnd.assign(1, sm.pool_off);
-  e.kernelLaunches++;
-  if (withInit && sm.panic) { e.err = "initialisation panicked"; return sm.panic; }
+  CtaWords w = {};
+  e.packCtaWords(&w, 1, withInit);
+  runCta(e.dev, &sm, (const hived_event_t*)e.dEvents.p, n, (hived_result_t*)e.dResults.p,
+         e.hasSugg ? (const uint32_t*)e.dSugg.p : nullptr, e.hasAux ? (const int32_t*)e.dAux.p : nullptr,
+         withInit ? (const int32_t*)e.dInit.p : nullptr, e.nPinnedOrder, e.nBad, (int32_t*)e.dPool.p, &w, nullptr, nullptr, 0, 1);
+  if (int rc = e.takeCtaWords(&w, 1, withInit, 1)) { e.err = "initialisation panicked"; return rc; }
   return 0;
 }
 }  // namespace hived

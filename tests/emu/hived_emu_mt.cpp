@@ -67,27 +67,17 @@ int launchProgram(Engine& e, int n, bool withInit) {
     e.kernelLaunches++;
     return 0;
   }
-  std::vector<int32_t> stops(C, 0);
   std::vector<Sm> sms(C);
   memset((void*)sms.data(), 0, sizeof(Sm) * C);
-  std::vector<long long> poolEnd(C, 0);
-  std::vector<int> panics(C, 0);
+  CtaWords w[MAX_CTAS] = {};
+  e.packCtaWords(w, C, withInit);
   const int32_t* own = (C > 1 || mgMode) ? (const int32_t*)e.dOwn.p : nullptr;
-  const int32_t* ownOff = own ? own + n : nullptr;
   auto body = [&](int cta) {
     hv_tls_cta = cta;
-    Sm& sm = sms[cta];
-    sm.lead_k = -1;
-    sm.pool_off = withInit ? 0 : (mgMode ? e.mgPoolCur[cta] : e.poolBase[cta]);
-    Core core(e.dev, &sm, (int32_t*)e.dPool.p, withInit ? 0 : e.poolBase[cta + 1], C);
-    int nOwn = own ? ownOff[cta + 1] - ownOff[cta] : n;
-    if (mgMode) { core.setMultiGpu(mgMode, e.mgCursor[cta]); nOwn = e.mgLimit[cta]; }
-    core.run((const hived_event_t*)e.dEvents.p, n, (hived_result_t*)e.dResults.p, e.hasSugg ? (const uint32_t*)e.dSugg.p : nullptr,
-             e.hasAux ? (const int32_t*)e.dAux.p : nullptr, withInit ? (const int32_t*)e.dInit.p : nullptr, e.nPinnedOrder, e.nBad,
-             own ? own + ownOff[cta] : nullptr, nOwn);
-    stops[cta] = sm.stop_k;
-    poolEnd[cta] = sm.pool_off;
-    panics[cta] = sm.panic;
+    runCta(e.dev, &sms[cta], (const hived_event_t*)e.dEvents.p, n, (hived_result_t*)e.dResults.p,
+           e.hasSugg ? (const uint32_t*)e.dSugg.p : nullptr, e.hasAux ? (const int32_t*)e.dAux.p : nullptr,
+           withInit ? (const int32_t*)e.dInit.p : nullptr, e.nPinnedOrder, e.nBad, (int32_t*)e.dPool.p, w, own,
+           own ? own + n : nullptr, cta, C);
   };
   if (C == 1) {
     body(0);
@@ -103,11 +93,7 @@ int launchProgram(Engine& e, int n, bool withInit) {
     Core core(e.dev, &sm, nullptr, 0, 1);
     core.repairSharedAncestors();
   }
-  e.kernelLaunches += (C > 1 && !mgMode) ? 2 : 1;
-  e.poolEnd.assign(poolEnd.begin(), poolEnd.end());
-  if (mgMode) e.mgStopOut.assign(stops.begin(), stops.end());
-  e.poolOff = poolEnd[0];
-  if (withInit && panics[0]) { e.err = "initialisation panicked"; return panics[0]; }
+  if (int rc = e.takeCtaWords(w, C, withInit, (C > 1 && !mgMode) ? 2 : 1)) { e.err = "initialisation panicked"; return rc; }
   return 0;
 }
 }  // namespace hived

@@ -12,26 +12,23 @@ int bk_launch_many(Engine* const* es, int k) {
     Engine* e;
     int C;
     std::vector<Sm> sms;
+    CtaWords w[MAX_CTAS];
   };
   std::vector<Ctx> cs;
   for (int y = 0; y < k; y++) {
-    Ctx c{es[y], es[y]->launchCta, std::vector<Sm>(es[y]->launchCta)};
+    Ctx c{es[y], es[y]->launchCta, std::vector<Sm>(es[y]->launchCta), {}};
     memset((void*)c.sms.data(), 0, sizeof(Sm) * c.C);
+    es[y]->packCtaWords(c.w, c.C, false);
     cs.push_back(std::move(c));
   }
   auto body = [](Ctx* c, int cta) {  // launchProgram's CTA body of an ordinary (not initialising, not partitioned) run
     Engine& e = *c->e;
     const int n = e.stagedN;
     hv_tls_cta = cta;
-    Sm& sm = c->sms[cta];
-    sm.lead_k = -1;
-    sm.pool_off = e.poolBase[cta];
     const int32_t* own = c->C > 1 ? (const int32_t*)e.dOwn.p : nullptr;
-    const int32_t* ownOff = own ? own + n : nullptr;
-    Core core(e.dev, &sm, (int32_t*)e.dPool.p, e.poolBase[cta + 1], c->C);
-    core.run((const hived_event_t*)e.dEvents.p, n, (hived_result_t*)e.dResults.p, e.hasSugg ? (const uint32_t*)e.dSugg.p : nullptr,
-             e.hasAux ? (const int32_t*)e.dAux.p : nullptr, nullptr, e.nPinnedOrder, e.nBad, own ? own + ownOff[cta] : nullptr,
-             own ? ownOff[cta + 1] - ownOff[cta] : n);
+    runCta(e.dev, &c->sms[cta], (const hived_event_t*)e.dEvents.p, n, (hived_result_t*)e.dResults.p,
+           e.hasSugg ? (const uint32_t*)e.dSugg.p : nullptr, e.hasAux ? (const int32_t*)e.dAux.p : nullptr, nullptr, e.nPinnedOrder,
+           e.nBad, (int32_t*)e.dPool.p, c->w, own, own ? own + n : nullptr, cta, c->C);
   };
   std::vector<std::thread> th;
   for (auto& c : cs)
@@ -46,10 +43,7 @@ int bk_launch_many(Engine* const* es, int k) {
       Core core(e.dev, &sm, nullptr, 0, 1);
       core.repairSharedAncestors();
     }
-    e.kernelLaunches += c.C > 1 ? 2 : 1;
-    e.poolEnd.assign(c.C, 0);
-    for (int cta = 0; cta < c.C; cta++) e.poolEnd[cta] = c.sms[cta].pool_off;
-    e.poolOff = c.sms[0].pool_off;
+    e.takeCtaWords(c.w, c.C, false, c.C > 1 ? 2 : 1);
   }
   return 0;
 }

@@ -59,7 +59,7 @@ struct LaunchArgs {
   bool withInit;
   int C;
   Sm* sms;
-  long long* scal;
+  CtaWords* words;
   bool repair;
   int mgMode;
 };
@@ -74,18 +74,11 @@ static void kernelEntry(void* p) {
     core.repairSharedAncestors();
     return;
   }
-  if (simt::tid() == 0) { sm.cmd = CMD_IDLE; sm.panic = 0; sm.lead_k = -1; sm.pool_off = a.scal[cta * 4 + 0]; }
-  simt::cta_barrier();
-  Core core(e.dev, &sm, (int32_t*)e.dPool.p, a.scal[cta * 4 + 1], a.C);
   const int32_t* own = (a.C > 1 || a.mgMode) ? (const int32_t*)e.dOwn.p : nullptr;
-  const int32_t* ownOff = own ? own + a.n : nullptr;
-  int nOwn = own ? ownOff[cta + 1] - ownOff[cta] : a.n;
-  if (a.mgMode) { core.setMultiGpu(a.mgMode, e.mgCursor[cta]); nOwn = e.mgLimit[cta]; }
-  core.run((const hived_event_t*)e.dEvents.p, a.n, (hived_result_t*)e.dResults.p, e.hasSugg ? (const uint32_t*)e.dSugg.p : nullptr,
-           e.hasAux ? (const int32_t*)e.dAux.p : nullptr, a.withInit ? (const int32_t*)e.dInit.p : nullptr, e.nPinnedOrder, e.nBad,
-           own ? own + ownOff[cta] : nullptr, nOwn);
-  simt::cta_barrier();
-  if (simt::tid() == 0) { a.scal[cta * 4 + 0] = sm.pool_off; a.scal[cta * 4 + 2] = sm.panic; a.scal[cta * 4 + 3] = sm.stop_k; }
+  runCta(e.dev, &sm, (const hived_event_t*)e.dEvents.p, a.n, (hived_result_t*)e.dResults.p,
+         e.hasSugg ? (const uint32_t*)e.dSugg.p : nullptr, e.hasAux ? (const int32_t*)e.dAux.p : nullptr,
+         a.withInit ? (const int32_t*)e.dInit.p : nullptr, e.nPinnedOrder, e.nBad, (int32_t*)e.dPool.p, a.words, own,
+         own ? own + a.n : nullptr, cta, a.C);
 }
 
 int launchProgram(Engine& e, int n, bool withInit) {
@@ -95,29 +88,21 @@ int launchProgram(Engine& e, int n, bool withInit) {
   const int mgMode = withInit ? 0 : e.mgMode;
   std::vector<Sm> sms(C);
   memset((void*)sms.data(), 0, sizeof(Sm) * C);
-  long long scal[MAX_CTAS * 4] = {0};
+  CtaWords w[MAX_CTAS] = {};
   if (mgMode == 3) {
-    LaunchArgs r{&e, n, false, 1, sms.data(), scal, true, 0};
+    LaunchArgs r{&e, n, false, 1, sms.data(), w, true, 0};
     simt::launch(1, NT, kernelEntry, &r);
     e.kernelLaunches++;
     return 0;
   }
-  for (int c = 0; c < C; c++) {
-    scal[c * 4 + 0] = withInit ? 0 : (mgMode ? e.mgPoolCur[c] : e.poolBase[c]);
-    scal[c * 4 + 1] = withInit ? 0 : e.poolBase[c + 1];
-  }
-  LaunchArgs a{&e, n, withInit, C, sms.data(), scal, false, mgMode};
+  e.packCtaWords(w, C, withInit);
+  LaunchArgs a{&e, n, withInit, C, sms.data(), w, false, mgMode};
   simt::launch(C, NT, kernelEntry, &a);
   if (C > 1 && !mgMode) {
-    LaunchArgs r{&e, n, false, 1, sms.data(), scal, true, 0};
+    LaunchArgs r{&e, n, false, 1, sms.data(), w, true, 0};
     simt::launch(1, NT, kernelEntry, &r);
   }
-  e.kernelLaunches += (C > 1 && !mgMode) ? 2 : 1;
-  e.poolEnd.assign(C, 0);
-  for (int c = 0; c < C; c++) e.poolEnd[c] = scal[c * 4 + 0];
-  if (mgMode) { e.mgStopOut.assign(C, 0); for (int c = 0; c < C; c++) e.mgStopOut[c] = (int32_t)scal[c * 4 + 3]; }
-  e.poolOff = scal[0];
-  if (withInit && scal[2]) { e.err = "initialisation panicked"; return (int)scal[2]; }
+  if (int rc = e.takeCtaWords(w, C, withInit, (C > 1 && !mgMode) ? 2 : 1)) { e.err = "initialisation panicked"; return rc; }
   return 0;
 }
 }  // namespace hived

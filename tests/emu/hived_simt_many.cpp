@@ -26,15 +26,15 @@ int bk_launch_many(Engine* const* es, int k) {
   int NT = env ? atoi(env) : 96;
   if (NT < 32 || NT % 32 || NT > 32 * MAX_WARPS) NT = 96;
   std::vector<std::vector<Sm>> sms(k);
-  std::vector<std::vector<long long>> scal(k, std::vector<long long>(MAX_CTAS * 4, 0));
+  std::vector<std::vector<CtaWords>> words(k, std::vector<CtaWords>(MAX_CTAS));
   ManyLaunch m{{}, 1};
   for (int y = 0; y < k; y++) {
     Engine& e = *es[y];
     const int C = e.launchCta;
     sms[y].resize(C);
     memset((void*)sms[y].data(), 0, sizeof(Sm) * C);
-    for (int c = 0; c < C; c++) { scal[y][c * 4 + 0] = e.poolBase[c]; scal[y][c * 4 + 1] = e.poolBase[c + 1]; }
-    m.ctx.push_back(LaunchArgs{&e, e.stagedN, false, C, sms[y].data(), scal[y].data(), false, 0});
+    e.packCtaWords(words[y].data(), C, false);
+    m.ctx.push_back(LaunchArgs{&e, e.stagedN, false, C, sms[y].data(), words[y].data(), false, 0});
     if (C > m.cmax) m.cmax = C;
   }
   simt::launch(m.cmax * k, NT, manyEntry, &m);
@@ -42,13 +42,10 @@ int bk_launch_many(Engine* const* es, int k) {
     Engine& e = *es[y];
     const int C = e.launchCta;
     if (C > 1) {
-      LaunchArgs r{&e, e.stagedN, false, 1, sms[y].data(), scal[y].data(), true, 0};
+      LaunchArgs r{&e, e.stagedN, false, 1, sms[y].data(), words[y].data(), true, 0};
       simt::launch(1, NT, kernelEntry, &r);
     }
-    e.kernelLaunches += C > 1 ? 2 : 1;
-    e.poolEnd.assign(C, 0);
-    for (int c = 0; c < C; c++) e.poolEnd[c] = scal[y][c * 4 + 0];
-    e.poolOff = scal[y][0];
+    e.takeCtaWords(words[y].data(), C, false, C > 1 ? 2 : 1);
   }
   return 0;
 }
