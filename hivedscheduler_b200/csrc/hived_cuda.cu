@@ -599,9 +599,7 @@ static int serveCall(Engine& e, ServeChan& c, const hived_event_t* events, int n
   const bool hasSugg = suggPool != nullptr && suggWords > 0, hasAux = aux != nullptr && auxWords > 0;
   const long long cap = poolCap < c.poolCap ? poolCap : c.poolCap;
   e.notePriorities(events, n);
-  e.launchCta = 1;
-  e.hasSugg = hasSugg; e.hasAux = hasAux;
-  e.poolCapWords = poolCap; e.stagedN = n; e.stagedEvents = events; e.canonicalDone = false;
+  e.setStaged(events, n, poolCap, hasSugg, hasAux);
   volatile int32_t* s = c.slotHost;
   int32_t* pay = (int32_t*)(s + SERVE_EV_OFF);
   memcpy(pay, events, (size_t)n * sizeof(hived_event_t));
@@ -715,17 +713,13 @@ int bk_run_small(Engine& e, const hived_event_t* events, int n, const uint32_t* 
     stage.bytes = total * 2;
   }
   e.notePriorities(events, n);
-  e.launchCta = 1;
-  e.ownOff.assign(2, 0); e.ownOff[1] = n;
-  e.poolBase.assign(2, 0); e.poolBase[1] = poolCap;
+  e.setStaged(events, n, poolCap, hasSugg, hasAux);
   e.dEvents.ensure((size_t)n * sizeof(hived_event_t));
   e.dResults.ensure((size_t)n * sizeof(hived_result_t));
   e.dPool.ensure((size_t)(poolCap > 0 ? poolCap : 1) * 4);
   if (hasSugg) e.dSugg.ensure((size_t)suggWords * 4);
   if (hasAux) e.dAux.ensure((size_t)auxWords * 4);
   if (e.buffersFailed()) { e.err = "out of device memory while staging the call"; return HIVED_ERR_CAPACITY; }
-  e.hasSugg = hasSugg; e.hasAux = hasAux;
-  e.poolCapWords = poolCap; e.stagedN = n; e.stagedEvents = events; e.canonicalDone = false;
   char* h = stage.host;
   memcpy(h + oEv, events, (size_t)n * sizeof(hived_event_t));
   CtaWords* w = (CtaWords*)(h + oScal);

@@ -88,10 +88,13 @@ struct Engine {
   long long poolOff = 0;
   // ---- VC-parallel execution
   int nCtaMax = 1, launchCta = 1;
-  std::vector<int32_t> ownOff;          // [launchCta + 1] into the owner-sorted index list (device: dOwn)
+  std::vector<int32_t> ownHost;         // the owner-sorted event list of a partitioned batch (device: dOwn)
+  std::vector<int32_t> ownOff;          // [launchCta + 1] into ownHost (device: dOwn + stagedN)
   std::vector<long long> poolBase;      // [launchCta + 1] pool slice of every CTA
   std::vector<long long> poolEnd;       // [launchCta] first unused word of every slice after the run
-  std::vector<uint8_t> ownerOf;         // owner CTA of every event of the batch being prepared (MAX_CTAS <= 255)
+  std::vector<uint8_t> ownerOf;         // owner CTA of every event of the batch being staged; NO_OWNER: another rank's
+                                        // (MAX_CTAS < NO_OWNER)
+  static constexpr uint8_t NO_OWNER = 0xff;
   std::vector<char> nodeBadHost;        // host mirror of the node health (decides whether a batch may run VC-parallel)
   std::vector<int32_t> groupStamp;      // batch that last named a group id (the two-VCs check is per batch)
   int32_t batchStamp = 0;
@@ -214,6 +217,7 @@ struct Engine {
       dev.scratch = dsc;
     }
     groupVcHost.assign((size_t)S.maxGroups, -1);
+    groupStamp.assign((size_t)S.maxGroups, 0);
     nodeBadHost.assign(T.nNodes > 0 ? T.nNodes : 1, 1);  // every node starts bad (hived_algorithm.go:453-464)
     badCount = T.nNodes;
     // initial dynamic state (hived_algorithm.go:108-145, 365-409)
@@ -258,55 +262,22 @@ struct Engine {
   // group of VCs) only in the regime where VCs interact through nothing but the chain-wide free lists:
   // every node healthy, a single guaranteed priority ever used (so no preemption, no lazy preemption, no
   // opportunistic cells), no recovery calls, and only SCHEDULE / DELETE events with valid VC ids.
-  int prepare(const hived_event_t* events, int n, int64_t poolCap) {
-    launchCta = 1;
+  int prepare(const hived_event_t* events, int n, int64_t poolCap, bool sugg, bool aux) {
     batchStamp++;
-    if (groupStamp.size() != groupVcHost.size()) groupStamp.assign(groupVcHost.size(), 0);
     uint64_t mask = prioMaskHost;
     // `calm`: the regime; the batch runs VC-parallel when it is calm and large enough to be split
     const bool split = nCtaMax > 1 && n >= 256;
     bool calm = badCount == 0 && !everRecovered;
     // one pass over the events: regime flags, the owner CTA of every event and the pool words every owner may need
     const int C = nCtaMax < T.nVCs ? nCtaMax : T.nVCs;
-    std::vector<int32_t> cnt(C + 1, 0);
     std::vector<long long> need(C, 0);
     ownerOf.resize((size_t)(n > 0 ? n : 1));
     for (int i = 0; i < n; i++) {
-      const hived_event_t& ev = events[i];
-      if (ev.type == HIVED_EV_SCHEDULE || ev.type == Core::EV_SCHEDULE_ONLY || ev.type == Core::EV_ADD_ALLOCATED) {
-        int p = ev.spec.priority;
-        mask |= (p >= -1 && p < 62) ? (1ull << (p + 1)) : (1ull << 62);
-      }
-      if (ev.type != HIVED_EV_SCHEDULE && ev.type != HIVED_EV_DELETE_ALLOCATED) calm = false;
-      // the VC that owns the event: a SCHEDULE names it; a DELETE belongs to the VC its group was scheduled under
-      // (the event's own VC field is optional, hived.h).  A group id seen under two VCs, or an unknown one: sequential.
-      int evVc = ev.spec.vc;
-      const int g = ev.spec.group;
-      if (ev.type == HIVED_EV_SCHEDULE || ev.type == Core::EV_SCHEDULE_ONLY) {
-        if (g >= 0 && g < (int)groupVcHost.size() && ev.spec.vc >= 0 && ev.spec.vc < T.nVCs) {
-          // a group id that THIS batch has already used under another VC (ids are recycled, hived.h "Id lifetime": the
-          // old incarnation's release and the new one's creation would meet in the same table row on two CTAs)
-          if (groupStamp[g] == batchStamp && groupVcHost[g] >= 0 && groupVcHost[g] != ev.spec.vc) calm = false;
-          groupVcHost[g] = ev.spec.vc;
-          groupStamp[g] = batchStamp;
-        }
-      } else if (ev.type == HIVED_EV_DELETE_ALLOCATED) {
-        evVc = (g >= 0 && g < (int)groupVcHost.size()) ? groupVcHost[g] : -1;
-        if (evVc < 0) evVc = (ev.spec.vc >= 0 && ev.spec.vc < T.nVCs) ? ev.spec.vc : 0;  // unknown group: a no-op wherever it runs
-        if (g >= 0 && g < (int)groupStamp.size()) groupStamp[g] = batchStamp;
-      }
-      if (evVc < 0 || evVc >= T.nVCs) calm = false;
-      if (ev.type == Core::EV_ADD_ALLOCATED) everRecovered = true;
+      const Route r = route(events[i], mask, nullptr);
+      if (!r.calmType || r.twoVcs || r.vc < 0) calm = false;
       if (split && calm) {
-        int o = evVc % C;
-        ownerOf[i] = (uint8_t)o;
-        cnt[o + 1]++;
-        if (ev.type == HIVED_EV_SCHEDULE) {
-          long long leaves = 0;
-          for (int m = 0; m < ev.spec.n_members && m < HIVED_MAX_MEMBERS; m++)
-            leaves += (long long)ev.spec.member_leaf_num[m] * ev.spec.member_pod_num[m];
-          need[o] += 3 * leaves;
-        }
+        ownerOf[i] = (uint8_t)(r.vc % C);
+        need[r.vc % C] += r.need;
       }
     }
     prioMaskHost = mask;
@@ -316,25 +287,13 @@ struct Engine {
     const char* noCalm = getenv("HIVED_NO_CALM");
     if (noCalm && *noCalm && *noCalm != '0') calm = false;
     dev.calm = calm ? 1 : 0;
-    ownOff.assign(2, 0); ownOff[1] = n;
-    poolBase.assign(2, 0); poolBase[1] = poolCap;
+    setStaged(events, n, poolCap, sugg, aux);
     if (simple) {
       long long total = 0;
       for (int c = 0; c < C; c++) total += need[c];
       if (total <= poolCap) {
-        launchCta = C;
-        ownOff.assign(C + 1, 0);
-        for (int c = 0; c < C; c++) ownOff[c + 1] = ownOff[c] + cnt[c + 1];
-        std::vector<int32_t> own(n), fill(ownOff.begin(), ownOff.end() - 1);
-        for (int i = 0; i < n; i++) own[fill[ownerOf[i]]++] = i;
-        dOwn.ensure((size_t)(n + C + 2) * 4);
-        bk_h2d(dOwn.p, own.data(), (size_t)n * 4);
-        bk_h2d((int32_t*)dOwn.p + n, ownOff.data(), (size_t)(C + 1) * 4);
-        poolBase.assign(C + 1, 0);
-        for (int c = 0; c < C; c++) poolBase[c + 1] = poolBase[c] + need[c];
-        std::vector<int32_t> prog(MAX_CTAS, 0x7fffffff);
-        for (int c = 0; c < C; c++) if (ownOff[c + 1] > ownOff[c]) prog[c] = own[ownOff[c]];
-        bk_h2d(dev.progress, prog.data(), MAX_CTAS * 4);
+        partition(n, C, need.data());
+        armProgress();
         multiBatches++;
       }
     }
@@ -342,10 +301,83 @@ struct Engine {
     dResults.ensure((size_t)(n > 0 ? n : 1) * sizeof(hived_result_t));
     dPool.ensure((size_t)(poolCap > 0 ? poolCap : 1) * 4);
     if (n > 0) bk_h2d(dEvents.p, events, (size_t)n * sizeof(hived_event_t));
-    poolCapWords = poolCap;
-    stagedN = n;
-    stagedEvents = events;
     return 0;
+  }
+  // The host's rule for one event (DESIGN.md §4), for every path that stages or runs events: its owning VC and what
+  // decides whether its batch is calm.  It updates the host state those decisions read: the priority mask `mask`,
+  // everRecovered and the group -> VC map (groupVcHost, stamped with batchStamp; `undo`, when given, receives the old
+  // value of every entry it writes).
+  struct Route {
+    int vc;          // the VC that owns the event, -1 when it names no valid one
+    bool calmType;   // a SCHEDULE or a DELETE_ALLOCATED: the only types a calm batch holds
+    bool twoVcs;     // a SCHEDULE of a group id this batch already used under another VC
+    long long need;  // the pool words a SCHEDULE may append: 3 x its leaves
+  };
+  Route route(const hived_event_t& ev, uint64_t& mask, std::vector<std::pair<int, int32_t>>* undo) {
+    Route r{ev.spec.vc, ev.type == HIVED_EV_SCHEDULE || ev.type == HIVED_EV_DELETE_ALLOCATED, false, 0};
+    if (ev.type == HIVED_EV_SCHEDULE || ev.type == Core::EV_SCHEDULE_ONLY || ev.type == Core::EV_ADD_ALLOCATED) {
+      int p = ev.spec.priority;
+      mask |= (p >= -1 && p < 62) ? (1ull << (p + 1)) : (1ull << 62);
+    }
+    if (ev.type == Core::EV_ADD_ALLOCATED) everRecovered = true;
+    // a SCHEDULE names its VC; a DELETE belongs to the VC its group was last scheduled under (the event's own VC field
+    // is optional, hived.h)
+    const int g = ev.spec.group;
+    const bool known = g >= 0 && g < (int)groupVcHost.size();
+    if (ev.type == HIVED_EV_SCHEDULE || ev.type == Core::EV_SCHEDULE_ONLY) {
+      if (known && ev.spec.vc >= 0 && ev.spec.vc < T.nVCs) {
+        // a group id that THIS batch has already used under another VC (ids are recycled, hived.h "Id lifetime": the
+        // old incarnation's release and the new one's creation would meet in the same table row on two CTAs)
+        r.twoVcs = groupStamp[g] == batchStamp && groupVcHost[g] >= 0 && groupVcHost[g] != ev.spec.vc;
+        if (undo) undo->push_back({g, groupVcHost[g]});
+        groupVcHost[g] = ev.spec.vc;
+        groupStamp[g] = batchStamp;
+      }
+    } else if (ev.type == HIVED_EV_DELETE_ALLOCATED) {
+      r.vc = known ? groupVcHost[g] : -1;
+      if (r.vc < 0) r.vc = (ev.spec.vc >= 0 && ev.spec.vc < T.nVCs) ? ev.spec.vc : 0;  // unknown group: a no-op wherever it runs
+      if (known) groupStamp[g] = batchStamp;
+    }
+    if (r.vc < 0 || r.vc >= T.nVCs) r.vc = -1;
+    if (ev.type == HIVED_EV_SCHEDULE)
+      for (int m = 0; m < ev.spec.n_members && m < HIVED_MAX_MEMBERS; m++)
+        r.need += 3 * (long long)ev.spec.member_leaf_num[m] * ev.spec.member_pod_num[m];
+    return r;
+  }
+  // Lay a batch out on C CTAs: the events with ownerOf[i] < C in C owner lists in event order (ownHost, ownOff), owner
+  // c's pool slice of need[c] words (poolBase), and both lists on the device (dOwn: the events, then the offsets).
+  void partition(int n, int C, const long long* need) {
+    launchCta = C;
+    ownOff.assign(C + 1, 0);
+    for (int i = 0; i < n; i++) if (ownerOf[i] < C) ownOff[ownerOf[i] + 1]++;
+    for (int c = 0; c < C; c++) ownOff[c + 1] += ownOff[c];
+    ownHost.resize(ownOff[C]);
+    std::vector<int32_t> fill(ownOff.begin(), ownOff.end() - 1);
+    for (int i = 0; i < n; i++) if (ownerOf[i] < C) ownHost[fill[ownerOf[i]]++] = i;
+    poolBase.assign(C + 1, 0);
+    for (int c = 0; c < C; c++) poolBase[c + 1] = poolBase[c] + need[c];
+    dOwn.ensure((size_t)(n + C + 2) * 4);
+    if (!ownHost.empty()) bk_h2d(dOwn.p, ownHost.data(), ownHost.size() * 4);
+    bk_h2d((int32_t*)dOwn.p + n, ownOff.data(), (size_t)(C + 1) * 4);
+  }
+  // the progress word of every CTA of a partitioned run starts at its first event (a run consumes them)
+  void armProgress() {
+    std::vector<int32_t> prog(MAX_CTAS, 0x7fffffff);
+    for (int c = 0; c < launchCta; c++) if (ownOff[c + 1] > ownOff[c]) prog[c] = ownHost[ownOff[c]];
+    bk_h2d(dev.progress, prog.data(), MAX_CTAS * 4);
+  }
+  // What the staged batch is: its n events, the caller's pool capacity, whether suggested-node and aux words were
+  // uploaded, and one CTA over the whole pool until partition() lays it out on more
+  void setStaged(const hived_event_t* events, int n, int64_t poolCap, bool sugg, bool aux) {
+    stagedEvents = events;
+    stagedN = n;
+    poolCapWords = poolCap;
+    hasSugg = sugg;
+    hasAux = aux;
+    canonicalDone = false;
+    launchCta = 1;
+    ownOff.assign(2, 0); ownOff[1] = n;
+    poolBase.assign(2, 0); poolBase[1] = poolCap;
   }
   // health events change the host mirror (applied after the batch ran)
   void trackHealth(const hived_event_t* events, int n) {
@@ -408,13 +440,10 @@ struct Engine {
   // the general path's staging (n > 0): prepare() + the suggested-node and aux words to the device
   int stageBatch(const hived_event_t* events, int n, const uint32_t* suggPool, int64_t suggWords, const int32_t* aux,
                  int64_t auxWords, int64_t poolCap) {
-    prepare(events, n, poolCap);
-    hasSugg = suggPool != nullptr && suggWords > 0;
+    prepare(events, n, poolCap, suggPool != nullptr && suggWords > 0, aux != nullptr && auxWords > 0);
     if (hasSugg) { dSugg.ensure((size_t)suggWords * 4); bk_h2d(dSugg.p, suggPool, (size_t)suggWords * 4); }
-    hasAux = aux != nullptr && auxWords > 0;
     if (hasAux) { dAux.ensure((size_t)auxWords * 4); bk_h2d(dAux.p, aux, (size_t)auxWords * 4); }
     poolOff = 0;
-    canonicalDone = false;
     if (buffersFailed()) { err = "out of device memory while staging the batch"; return HIVED_ERR_CAPACITY; }
     return 0;
   }
@@ -440,19 +469,9 @@ struct Engine {
     return 0;
   }
   static constexpr int SMALL_BATCH = 8;
-  // what prepare() decides per event, for bk_run_small (no device traffic)
+  // the host mirror after events that bk_run_small runs without prepare()
   void notePriorities(const hived_event_t* events, int n) {
-    for (int i = 0; i < n; i++) {
-      const hived_event_t& ev = events[i];
-      if (ev.type == HIVED_EV_SCHEDULE || ev.type == Core::EV_SCHEDULE_ONLY || ev.type == Core::EV_ADD_ALLOCATED) {
-        int p = ev.spec.priority;
-        prioMaskHost |= (p >= -1 && p < 62) ? (1ull << (p + 1)) : (1ull << 62);
-      }
-      if (ev.type == Core::EV_ADD_ALLOCATED) everRecovered = true;
-      if ((ev.type == HIVED_EV_SCHEDULE || ev.type == Core::EV_SCHEDULE_ONLY) && ev.spec.group >= 0 &&
-          ev.spec.group < (int)groupVcHost.size() && ev.spec.vc >= 0 && ev.spec.vc < T.nVCs)
-        groupVcHost[ev.spec.group] = ev.spec.vc;
-    }
+    for (int i = 0; i < n; i++) route(events[i], prioMaskHost, nullptr);
   }
   bool buffersFailed() const {
     return dEvents.failed || dResults.failed || dPool.failed || dSugg.failed || dAux.failed || dInit.failed || dScalars.failed ||
@@ -464,8 +483,7 @@ struct Engine {
   int stagedN = 0;
   int stage(const hived_event_t* events, int n, int64_t poolCap) {
     bk_use_device(deviceOrdinal);
-    hasSugg = false; hasAux = false;
-    return prepare(events, n, poolCap);
+    return prepare(events, n, poolCap, false, false);
   }
   int runStaged() {
     rearmStaged();
@@ -475,12 +493,7 @@ struct Engine {
     bk_use_device(deviceOrdinal);
     poolOff = 0;
     canonicalDone = false;
-    if (launchCta > 1) {  // the progress words were consumed by the previous run
-      std::vector<int32_t> own(stagedN), prog(MAX_CTAS, 0x7fffffff);
-      bk_d2h(own.data(), dOwn.p, (size_t)stagedN * 4);
-      for (int c = 0; c < launchCta; c++) if (ownOff[c + 1] > ownOff[c]) prog[c] = own[ownOff[c]];
-      bk_h2d(dev.progress, prog.data(), MAX_CTAS * 4);
-    }
+    if (launchCta > 1) armProgress();
   }
   // The launch words of the next run's C CTAs (hived_dev.h CtaWords; the initialisation runs one CTA without a pool)
   void packCtaWords(CtaWords* w, int C, bool withInit) const {
@@ -512,7 +525,7 @@ struct Engine {
   // events up to the first one that may touch them (mgRun), the ranks agree on the smallest such event (min over
   // ranks: the caller's collective), its owner runs it alone (mgSolo) and ships the arrays to everybody else.
   int mgMode = 0, mgRank = 0, mgWorld = 1;
-  std::vector<int32_t> mgCursor, mgLimit, mgStopOut, mgOwnHost;
+  std::vector<int32_t> mgCursor, mgLimit, mgStopOut;
   std::vector<long long> mgPoolCur;
   std::vector<std::pair<void*, size_t>> sharedArrays() {
     std::vector<std::pair<void*, size_t>> v;
@@ -543,12 +556,10 @@ struct Engine {
     if (world < 1 || rank < 0 || rank >= world) { err = "multi-GPU partition: bad rank/world"; return HIVED_ERR_BAD_SPEC; }
     if (badCount != 0 || everRecovered) { err = "multi-GPU partition: only calm batches (every node healthy, no recovery)"; return HIVED_ERR_BAD_SPEC; }
     batchStamp++;
-    if (groupStamp.size() != groupVcHost.size()) groupStamp.assign(groupVcHost.size(), 0);
     uint64_t mask = prioMaskHost;
     const int C = (T.nVCs - rank + world - 1) / world > 0 ? (T.nVCs - rank + world - 1) / world : 0;
     if (C > MAX_CTAS) { err = "multi-GPU partition: more VCs per rank than CTAs"; return HIVED_ERR_CAPACITY; }
     const int CL = C > 0 ? C : 1;
-    std::vector<std::vector<int32_t>> lists(CL);
     std::vector<long long> need(CL, 0);
     // a refused batch changes nothing: the group -> VC entries it wrote are put back
     std::vector<std::pair<int, int32_t>> undo;
@@ -557,62 +568,32 @@ struct Engine {
       err = why;
       return code;
     };
+    ownerOf.resize((size_t)(n > 0 ? n : 1));
     for (int i = 0; i < n; i++) {
       const hived_event_t& ev = events[i];
       if (ev.type != HIVED_EV_SCHEDULE && ev.type != HIVED_EV_DELETE_ALLOCATED) return refuse(HIVED_ERR_BAD_SPEC, "multi-GPU partition: only SCHEDULE / DELETE_ALLOCATED events");
       // no rank holds a suggested-node pool: such an event would silently see every node as suggested
       if (ev.suggested_off >= 0) return refuse(HIVED_ERR_BAD_SPEC, "multi-GPU partition: events with a suggested-node set are not supported");
-      int evVc = ev.spec.vc;
-      const int g = ev.spec.group;
-      if (ev.type == HIVED_EV_SCHEDULE) {
-        int p = ev.spec.priority;
-        mask |= (p >= -1 && p < 62) ? (1ull << (p + 1)) : (1ull << 62);
-        if (g >= 0 && g < (int)groupVcHost.size() && evVc >= 0 && evVc < T.nVCs) {
-          if (groupStamp[g] == batchStamp && groupVcHost[g] >= 0 && groupVcHost[g] != evVc) return refuse(HIVED_ERR_BAD_SPEC, "multi-GPU partition: a group id used under two VCs in one batch");
-          undo.push_back({g, groupVcHost[g]});
-          groupVcHost[g] = evVc;
-          groupStamp[g] = batchStamp;
-        }
-      } else {
-        if (g >= 0 && g < (int)groupStamp.size()) groupStamp[g] = batchStamp;
-        evVc = (g >= 0 && g < (int)groupVcHost.size()) ? groupVcHost[g] : -1;
-        if (evVc < 0) evVc = (ev.spec.vc >= 0 && ev.spec.vc < T.nVCs) ? ev.spec.vc : 0;
-      }
-      if (evVc < 0 || evVc >= T.nVCs) return refuse(HIVED_ERR_BAD_SPEC, "multi-GPU partition: event with an unknown VC");
-      if (evVc % world != rank) continue;
-      const int c = evVc / world;
-      lists[c].push_back(i);
-      if (ev.type == HIVED_EV_SCHEDULE) {
-        long long leaves = 0;
-        for (int m = 0; m < ev.spec.n_members && m < HIVED_MAX_MEMBERS; m++) leaves += (long long)ev.spec.member_leaf_num[m] * ev.spec.member_pod_num[m];
-        need[c] += 3 * leaves;
-      }
+      const Route r = route(ev, mask, &undo);
+      if (r.twoVcs) return refuse(HIVED_ERR_BAD_SPEC, "multi-GPU partition: a group id used under two VCs in one batch");
+      if (r.vc < 0) return refuse(HIVED_ERR_BAD_SPEC, "multi-GPU partition: event with an unknown VC");
+      const bool mine = r.vc % world == rank;
+      ownerOf[i] = mine ? (uint8_t)(r.vc / world) : NO_OWNER;
+      if (mine) need[r.vc / world] += r.need;
     }
     if ((mask & (mask - 1)) != 0 || (mask & 1)) return refuse(HIVED_ERR_BAD_SPEC, "multi-GPU partition: more than one priority in use");
     long long needAll = 0;
     for (int c = 0; c < CL; c++) needAll += need[c];
     if (needAll > poolCap) return refuse(HIVED_ERR_CAPACITY, "multi-GPU partition: pool too small");
     prioMaskHost = mask;
-    launchCta = CL;
-    ownOff.assign(CL + 1, 0);
-    mgOwnHost.clear();
-    for (int c = 0; c < CL; c++) { mgOwnHost.insert(mgOwnHost.end(), lists[c].begin(), lists[c].end()); ownOff[c + 1] = (int32_t)mgOwnHost.size(); }
-    poolBase.assign(CL + 1, 0);
-    for (int c = 0; c < CL; c++) poolBase[c + 1] = poolBase[c] + need[c];
-    dOwn.ensure((size_t)(n + CL + 2) * 4);
-    if (!mgOwnHost.empty()) bk_h2d(dOwn.p, mgOwnHost.data(), mgOwnHost.size() * 4);
-    bk_h2d((int32_t*)dOwn.p + n, ownOff.data(), (size_t)(CL + 1) * 4);
+    setStaged(events, n, poolCap, false, false);
+    partition(n, CL, need.data());
     dEvents.ensure((size_t)(n > 0 ? n : 1) * sizeof(hived_event_t));
     dResults.ensure((size_t)(n > 0 ? n : 1) * sizeof(hived_result_t));
     dPool.ensure((size_t)(poolCap > 0 ? poolCap : 1) * 4);
     if (buffersFailed()) { err = "out of device memory while staging the batch"; return HIVED_ERR_CAPACITY; }
     if (n > 0) bk_h2d(dEvents.p, events, (size_t)n * sizeof(hived_event_t));
     bk_zero(dResults.p, (size_t)(n > 0 ? n : 1) * sizeof(hived_result_t));  // events of other ranks stay all-zero here
-    poolCapWords = poolCap;
-    stagedN = n;
-    stagedEvents = events;
-    hasSugg = false; hasAux = false;
-    canonicalDone = false;
     mgRank = rank; mgWorld = world;
     mgCursor.assign(CL, 0);
     mgPoolCur.assign(poolBase.begin(), poolBase.end() - 1);
@@ -633,7 +614,7 @@ struct Engine {
     int mn = 0x7fffffff;
     for (int c = 0; c < launchCta; c++) {
       const int k = mgCursor[c], cnt = ownOff[c + 1] - ownOff[c];
-      if (k < cnt && mgOwnHost[ownOff[c] + k] < mn) mn = mgOwnHost[ownOff[c] + k];
+      if (k < cnt && ownHost[ownOff[c] + k] < mn) mn = ownHost[ownOff[c] + k];
     }
     return mn;
   }
@@ -655,7 +636,7 @@ struct Engine {
     mgLimit.assign(launchCta, 0);
     bool work = false;
     for (int c = 0; c < launchCta; c++) {
-      const int32_t* lst = mgOwnHost.data() + ownOff[c];
+      const int32_t* lst = ownHost.data() + ownOff[c];
       const int cnt = ownOff[c + 1] - ownOff[c];
       mgLimit[c] = (int32_t)(std::lower_bound(lst, lst + cnt, horizon) - lst);  // events of the list with index < horizon
       if (mgLimit[c] < mgCursor[c]) mgLimit[c] = mgCursor[c];
@@ -667,7 +648,7 @@ struct Engine {
     }
     int mn = 0x7fffffff;
     for (int c = 0; c < launchCta; c++)
-      if (mgCursor[c] < mgLimit[c] && mgOwnHost[ownOff[c] + mgCursor[c]] < mn) mn = mgOwnHost[ownOff[c] + mgCursor[c]];  // parked
+      if (mgCursor[c] < mgLimit[c] && ownHost[ownOff[c] + mgCursor[c]] < mn) mn = ownHost[ownOff[c] + mgCursor[c]];  // parked
     *stopEvent = mn;
     return 0;
   }
@@ -678,7 +659,7 @@ struct Engine {
     int owner = -1;
     for (int c = 0; c < launchCta; c++) {
       const int k = mgCursor[c], cnt = ownOff[c + 1] - ownOff[c];
-      if (k < cnt && mgOwnHost[ownOff[c] + k] == eventIndex) { owner = c; break; }
+      if (k < cnt && ownHost[ownOff[c] + k] == eventIndex) { owner = c; break; }
     }
     if (owner < 0) { err = "multi-GPU partition: this rank is not stopped at that event"; return HIVED_ERR_BAD_SPEC; }
     mgLimit[owner] = mgCursor[owner] + 1;

@@ -76,15 +76,6 @@ def _check(lib, ctx, rc: int, what: str) -> None:
         raise RuntimeError("%s failed: rc=%d %s" % (what, rc, msg.decode() if msg else ""))
 
 
-def event_owner(events, i: int, group_vc: dict, world: int) -> int:
-    """Rank that owns event i (SCHEDULE: its VC; DELETE: the VC its group was scheduled under)."""
-    ev = events[i]
-    if ev.type == _cabi.EV_SCHEDULE:
-        group_vc[ev.spec.group] = ev.spec.vc
-        return ev.spec.vc % world
-    return group_vc.get(ev.spec.group, max(ev.spec.vc, 0)) % world
-
-
 def run_partitioned(lib: C.CDLL, ctx, events, n: int, pool_cap: int, rank: int, world: int, device: Optional[str] = None,
                     staged: bool = False, window: Optional[int] = None) -> dict:
     """Drive one partitioned batch on this rank (collective: every rank of the process group calls it with the same

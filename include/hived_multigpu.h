@@ -31,7 +31,7 @@
  * touch the cluster-wide state: the sequential contract holds, results are identical to a single-GPU run (the
  * chain hash over the merged results — hived_mg_chain_hash — is the witness).  Only calm batches are accepted
  * (SCHEDULE / DELETE_ALLOCATED events, every node healthy, one guaranteed priority, no recovery): the regime in
- * which the single-GPU engine runs VC-parallel (hived_engine.hpp prepare()).  hived_mg_stage refuses with
+ * which the single-GPU engine runs VC-parallel (hived_engine.hpp Engine::route).  hived_mg_stage refuses with
  * HIVED_ERR_BAD_SPEC, and changes nothing, a batch with any other event type, an event with a suggested-node set
  * (suggested_off >= 0: no rank holds a suggested-node pool), more than one priority (or an opportunistic one), a
  * group id scheduled under two VCs, or an event of an unknown VC; and any batch on a context with a bad node or a

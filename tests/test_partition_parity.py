@@ -166,7 +166,7 @@ class Ranks:
             res, pool, _ = dist.fetch_results(lib, bc.ctx, n, cap)
             fetched.append((res, pool))
         owners = np.zeros(n, dtype=np.int64)
-        for i in range(n):  # hived_engine.hpp mgStage's routing (dist.event_owner)
+        for i in range(n):  # the routing of hived_engine.hpp Engine::route
             g, v = int(ev["spec"]["group"][i]), int(ev["spec"]["vc"][i])
             if ev["type"][i] == _cabi.EV_SCHEDULE:
                 self.group_vc[g] = v
