@@ -2761,14 +2761,22 @@ struct Core {
     if (thisOff < 0) { panic(HIVED_ERR_PLATFORM); return; }
     int first = phys[thisOff];
     if (bad) ST(res->incomplete, 1);
-    lastLeafOff = base;
     int firstReal = first;  // PodPlacementInfo.PhysicalNode comes from the pod's first cell that still exists
     if (bad && first < 0) {
       int j = firstIdx(thisN, [&](int q) { return phys[thisOff + q] >= 0; });
       firstReal = j >= 0 ? phys[thisOff + j] : -1;
     }
-    lastNode = firstReal >= 0 ? d.p_node[firstReal] : -1; lastChain = first >= 0 ? d.p_chain[first] : -1;
-    lastFirstLeaf = first >= 0 ? d.p_leafidx[first] : -1;
+    bindRecord(res, base, nl, nmem, memLeaf, memPods, hasVirtual, curPodIndex, thisOff, thisN,
+               firstReal >= 0 ? d.p_node[firstReal] : -1, first >= 0 ? d.p_chain[first] : -1,
+               first >= 0 ? d.p_leafidx[first] : -1);
+  }
+  // the end of emitBind once the pool triples are written: the bind's fixed record fields and last* state, and the
+  // pool's next free word.  node / chain / firstLeaf: the pod's physical node, and the chain and leaf index of its
+  // first cell
+  HIVED_DEV void bindRecord(hived_result_t* res, long long base, int nl, int nmem, const int* memLeaf, const int* memPods,
+                            bool hasVirtual, int curPodIndex, int thisOff, int thisN, int node, int chain, int firstLeaf) {
+    lastLeafOff = base;
+    lastNode = node; lastChain = chain; lastFirstLeaf = firstLeaf;
     lastKind = HIVED_KIND_BIND; lastHasVirtual = hasVirtual ? 1 : 0; lastNmem = nmem;
     for (int m = 0; m < nmem; m++) { lastMemLeaf[m] = memLeaf[m]; lastMemPods[m] = memPods[m]; }
     if (lane == 0) {  // the fixed part of the record, one sequence point
