@@ -144,6 +144,13 @@ def bind_many(lib: C.CDLL) -> C.CDLL:
     return lib
 
 
+def bind_clone(lib: C.CDLL) -> C.CDLL:
+    """Type hived_clone (include/hived_clone.h) on a library loaded with load_library."""
+    lib.hived_clone.restype = C.c_int
+    lib.hived_clone.argtypes = [_P, C.c_int32, C.c_int32, C.POINTER(_P)]
+    return lib
+
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 CUDA_LIB_PATH = os.path.join(_HERE, "csrc", "libhived_cuda.so")
 

@@ -264,6 +264,34 @@ class HivedAlgorithm:
         except Exception:
             pass
 
+    def clone(self, device: Optional[int] = None, concurrent: bool = False) -> "HivedAlgorithm":
+        """A second scheduler that answers every later call exactly as this one would (include/hived_clone.h), for
+        what-if runs: the library's state is copied into a new context (``device``: its CUDA ordinal, default this
+        one's; ``concurrent``: HIVED_OPT_CONCURRENT), and the state this shim keeps above the ABI — the name <-> id
+        tables with their recycled ids, the pod objects it keeps for victims and missing placements, the random
+        state that picks a preemption's node — is copied too.  The two share nothing afterwards."""
+        flags = (int(self._opt.flags) & ~_cabi.OPT_CONCURRENT) | (_cabi.OPT_CONCURRENT if concurrent else 0)
+        ctx = C.c_void_p()
+        rc = _cabi.bind_clone(self._lib).hived_clone(self._ctx, -1 if device is None else device, flags, C.byref(ctx))
+        if rc != 0:
+            raise PlatformError("hived_clone failed (%d): %s" % (rc, (self._lib.hived_create_error() or b"").decode()))
+        h = copy.copy(self)  # the cluster's name tables, shared read-only
+        h._ctx = ctx
+        h._opt = _cabi.Options.from_buffer_copy(self._opt)
+        h._opt.flags = flags
+        if device is not None:
+            h._opt.device = device
+        h._groups, h._pods = copy.deepcopy(self._groups), copy.deepcopy(self._pods)
+        h._pod_objs = dict(self._pod_objs)
+        h._pool = (C.c_int32 * self._pool_cap)()
+        h._rand = random.Random()
+        h._rand.setstate(self._rand.getstate())
+        h._ingest = None
+        if self._ingest is not None:
+            from .ingest import Ingest
+            h._ingest = Ingest(self._lib, ctx)
+        return h
+
     # ---------------------------------------------------------------- helpers
     @property
     def backend(self) -> str:

@@ -15,6 +15,7 @@
 
 #define HIVED_BK_LAUNCH_MANY 1  // the joint launch below
 #define HIVED_BK_CONCURRENT 1   // concurrent contexts' own resident kernels and batches below
+#define HIVED_BK_COPY_CTX 1     // hived_clone's copies on the clone's stream below
 #include "hived_engine.hpp"
 #include "hived_many.h"
 #include "hived_seats.h"
@@ -392,20 +393,27 @@ static int launchDone(Engine* const* es, int k, CudaTimers* t, cudaStream_t st, 
   return 0;
 }
 
-int launchProgram(Engine& e, int n, bool withInit) {
-  // a concurrent context's batch: its own stream, constant slot and seats, no turn
-  if (t_own && e.stream && t_own == ((CudaTimers*)e.stream)->conc && !withInit && !e.mgMode) return concLaunch(e, *t_own, n);
-  Turn turn(e);
+// The context's stream and timing events, made by its first launch (or, for a clone, its first copy) with its device
+// current; nullptr with e.err set if the stream cannot be created.
+static CudaTimers* timersOf(Engine& e) {
   if (!e.stream) {
     // the kernel wants L1, not shared memory: ask for the smallest carveout that holds its ~18 KB of static smem
     cudaFuncSetAttribute(hived_events_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 10);
     CudaTimers* t = new CudaTimers();
-    if (!cudaOk(cudaStreamCreate(&t->stream), e.err, "cudaStreamCreate")) return HIVED_ERR_NO_DEVICE;
+    if (!cudaOk(cudaStreamCreate(&t->stream), e.err, "cudaStreamCreate")) return nullptr;
     cudaEventCreate(&t->start);
     cudaEventCreate(&t->stop);
     e.stream = t;
   }
-  CudaTimers* t = (CudaTimers*)e.stream;
+  return (CudaTimers*)e.stream;
+}
+
+int launchProgram(Engine& e, int n, bool withInit) {
+  // a concurrent context's batch: its own stream, constant slot and seats, no turn
+  if (t_own && e.stream && t_own == ((CudaTimers*)e.stream)->conc && !withInit && !e.mgMode) return concLaunch(e, *t_own, n);
+  Turn turn(e);
+  CudaTimers* t = timersOf(e);
+  if (!t) return HIVED_ERR_NO_DEVICE;
   bk_quiesce(e);
   if (int rc = takeCopyError(e.err)) return rc;  // a staging copy of this batch (or of create()) failed
   if (int rc = ensureDevLoaded(e)) return rc;
@@ -494,6 +502,35 @@ bool bk_batch_begin(Engine& e) {
   return true;
 }
 void bk_batch_end(Engine&) { t_own = nullptr; }
+
+// ---- hived_clone (include/hived_clone.h) ---------------------------------------------------------------------------
+// The copies are queued on the clone's stream (copy engines; a peer copy when the clone lives on another device, which
+// needs no peer access) and waited for once.  Ordering with the source: the caller holds `src`, so none of its calls is
+// in flight.  Each of them ended either in a synchronisation of the stream that ran it (batches, joint launches, the
+// per-call path without a resident kernel) or with the host observing the `done` word of a resident kernel, which the
+// kernel stores after flushing its counters and __threadfence_system(): either way every write of src's last call is
+// complete and visible to the copy engines.  A resident kernel of src that is still waiting for its next call writes
+// no device state until it gets one, so it is left running, and src is not touched.  No turn: the copies run on the
+// clone's own stream and read memory no other context writes.
+int bk_copy_ctx(Engine& dst, const Engine& src, void* const* to, const void* const* from, const size_t* bytes, int n) {
+  CudaTimers* t = timersOf(dst);  // dst's device is current (bk_init)
+  if (!t) return HIVED_ERR_NO_DEVICE;
+  if (int rc = takeCopyError(dst.err)) return rc;  // an upload of the static arrays failed
+  cudaError_t ce = cudaSuccess;
+  for (int i = 0; i < n && ce == cudaSuccess; i++) {
+    if (!bytes[i]) continue;
+    ce = dst.deviceOrdinal == src.deviceOrdinal
+             ? cudaMemcpyAsync(to[i], from[i], bytes[i], cudaMemcpyDeviceToDevice, t->stream)
+             : cudaMemcpyPeerAsync(to[i], dst.deviceOrdinal, from[i], src.deviceOrdinal, bytes[i], t->stream);
+  }
+  if (ce == cudaSuccess) ce = cudaStreamSynchronize(t->stream);
+  if (ce != cudaSuccess) {
+    cudaGetLastError();
+    dst.err = std::string("copying the source context's state failed: ") + cudaGetErrorString(ce);
+    return HIVED_ERR_PLATFORM;
+  }
+  return 0;
+}
 
 // ---- joint launches (include/hived_multictx.h, hived_cuda_many.cu) ------------------------------------------------
 // The staged batches of several contexts of one device run in one launch, each context on CTAs of its own, on the first

@@ -15,6 +15,7 @@
 #include <vector>
 
 #include "../../include/hived.h"
+#include "../../include/hived_clone.h"
 #include "../../include/hived_hash.h"
 #include "../../include/hived_multictx.h"
 #include "../../include/hived_multigpu.h"
@@ -59,6 +60,10 @@ int bk_open_concurrent(Engine& e);
 bool bk_batch_begin(Engine& e);
 void bk_batch_end(Engine& e);
 void bk_flush_l2();
+// hived_clone (include/hived_clone.h): n device regions of `src` into the new context `dst`, dst[i] <- from[i], bytes[i]
+// each, on dst's device (which may be another one than src's); 0, or HIVED_ERR_* with dst.err set.  A backend that
+// defines HIVED_BK_COPY_CTX before including this header supplies it; the others get the one below (bk_d2d per region).
+int bk_copy_ctx(Engine& dst, const Engine& src, void* const* to, const void* const* from, const size_t* bytes, int n);
 
 struct Buf {
   void* p = nullptr;
@@ -162,59 +167,16 @@ struct Engine {
       err = e.what();
       return HIVED_ERR_BAD_CONFIG;
     }
-    DevSizes& S = dev.S;
-    S.NP = T.NP; S.NV = T.NV; S.nChains = T.nChains; S.nVCs = T.nVCs; S.nLeafTypes = T.nLeafTypes; S.nPinned = T.nPinned;
-    S.nNodes = T.nNodes; S.nVsets = T.nVsets; S.nScheds = T.nScheds;
-    S.flTotal = T.flTotal; S.dmTotal = T.dmTotal; S.cvTotal = (int32_t)T.cv_init.size();
-    S.maxGroups = opt.max_groups; S.maxPods = opt.max_pods; S.LS = opt.max_group_leaves; S.PS = opt.max_group_pods;
-    S.VX = S.LS * MAXL + 16; S.LZ = S.LS < 64 ? S.LS : 64;
-    S.maxLevelCount = T.maxLevelCount; S.maxViewN = T.maxViewN; S.bitmapWords = (T.nNodes + 31) / 32;
-    S.maxLevels = T.maxLevels; S.maxNodeLeaves = T.maxNodeLeaves; S.AS = T.AS; S.directLeaf = T.uniqueLeafIdx ? 1 : 0;
-#define X(name) dev.name = uploadStatic(T.name);
-    HIVED_STATIC_ARRAYS(X)
-#undef X
-#define Y(name, count, init)                                                   \
-  {                                                                            \
-    size_t cnt_ = (size_t)(count);                                             \
-    dev.name = allocFill<int32_t>(cnt_, (int32_t)(init));                      \
-    mutableRegions.push_back({dev.name, (cnt_ ? cnt_ : 1) * sizeof(int32_t)}); \
-  }
-    HIVED_MUTABLE_ARRAYS(Y)
-#undef Y
-    auto oom = [&]() {
-      err = "out of device memory while creating the context (see hived_options_t: the group tables grow with "
-            "max_groups * max_group_leaves)";
-      return HIVED_ERR_CAPACITY;
-    };
-    if (allocFailed) return oom();  // before anything is copied into a null array
-    dev.g_state.b = dev.g_vc.b = dev.g_prio.b = dev.g_flags.b = dev.g_nmem.b = dev.g_npre.b = dev.g_hdr;
-    dev.g_mem_leaf.b = dev.g_mem_pods.b = dev.g_hdr;
+    // one private scratch set per CTA (VC-parallel execution uses up to nCtaMax CTAs)
+    nCtaMax = T.nVCs < 16 ? (T.nVCs > 0 ? T.nVCs : 1) : 16;
+    if (const char* env = getenv("HIVED_NCTA")) { int v = atoi(env); if (v >= 1 && v <= MAX_CTAS) nCtaMax = v < nCtaMax ? v : nCtaMax; }
+    rc = allocate(true);
+    if (rc) return rc;
+    const DevSizes& S = dev.S;
     {  // g_vc starts at -1
       std::vector<int32_t> hdr((size_t)(S.maxGroups + GHOST_GROUPS) * GROUP_HDR_WORDS, 0);
       for (int g = 0; g < S.maxGroups + GHOST_GROUPS; g++) hdr[(size_t)g * GROUP_HDR_WORDS + 1] = -1;
       bk_h2d(dev.g_hdr, hdr.data(), hdr.size() * 4);
-    }
-    dev.stats = allocFill<long long>(ST_COUNT, 0);
-    mutableRegions.push_back({dev.stats, ST_COUNT * sizeof(long long)});
-    dev.epoch = allocFill<int32_t>(MAX_CTAS, 1);
-    mutableRegions.push_back({dev.epoch, MAX_CTAS * sizeof(int32_t)});
-    dev.progress = allocFill<int32_t>(MAX_CTAS, 0);
-    if (allocFailed) return oom();
-    // one private scratch set per CTA (VC-parallel execution uses up to nCtaMax CTAs)
-    nCtaMax = T.nVCs < 16 ? (T.nVCs > 0 ? T.nVCs : 1) : 16;
-    if (const char* env = getenv("HIVED_NCTA")) { int v = atoi(env); if (v >= 1 && v <= MAX_CTAS) nCtaMax = v < nCtaMax ? v : nCtaMax; }
-    {
-      std::vector<Scratch> sc(nCtaMax);
-      for (int c = 0; c < nCtaMax; c++) {
-#define Z(name, count) sc[c].name = allocFill<int32_t>((size_t)(count), 0);
-        HIVED_SCRATCH_ARRAYS(Z)
-#undef Z
-      }
-      Scratch* dsc = (Scratch*)bk_alloc(sizeof(Scratch) * nCtaMax);
-      if (!dsc || allocFailed) { if (dsc) bk_free(dsc); return oom(); }
-      bk_h2d(dsc, sc.data(), sizeof(Scratch) * nCtaMax);
-      allocs.push_back(dsc);
-      dev.scratch = dsc;
     }
     groupVcHost.assign((size_t)S.maxGroups, -1);
     groupStamp.assign((size_t)S.maxGroups, 0);
@@ -241,19 +203,130 @@ struct Engine {
     nBad = (int)T.bad_init_order.size();
     dInit.ensure((init.size() + 1) * 4);
     if (!init.empty()) bk_h2d(dInit.p, init.data(), init.size() * 4);
+    poolOff = 0;
+    if (dInit.failed) return outOfMemory();
+    rc = launchProgram(*this, 0, true);
+    if (rc) { if (err.empty()) err = "device initialisation failed"; return rc; }
+    if (opt.flags & HIVED_OPT_CONCURRENT) return bk_open_concurrent(*this);
+    return 0;
+  }
+  int outOfMemory() {
+    err = "out of device memory while creating the context (see hived_options_t: the group tables grow with "
+          "max_groups * max_group_leaves)";
+    return HIVED_ERR_CAPACITY;
+  }
+  // The device half of a context that create() and cloneFrom() share: from T, opt and nCtaMax, the sizes, the static
+  // arrays (uploaded), the mutable arrays (`fill`: filled with their initial values; else left for the caller to
+  // write), the counters, the per-CTA scratch and the staging buffers.
+  int allocate(bool fill) {
+    DevSizes& S = dev.S;
+    S.NP = T.NP; S.NV = T.NV; S.nChains = T.nChains; S.nVCs = T.nVCs; S.nLeafTypes = T.nLeafTypes; S.nPinned = T.nPinned;
+    S.nNodes = T.nNodes; S.nVsets = T.nVsets; S.nScheds = T.nScheds;
+    S.flTotal = T.flTotal; S.dmTotal = T.dmTotal; S.cvTotal = (int32_t)T.cv_init.size();
+    S.maxGroups = opt.max_groups; S.maxPods = opt.max_pods; S.LS = opt.max_group_leaves; S.PS = opt.max_group_pods;
+    S.VX = S.LS * MAXL + 16; S.LZ = S.LS < 64 ? S.LS : 64;
+    S.maxLevelCount = T.maxLevelCount; S.maxViewN = T.maxViewN; S.bitmapWords = (T.nNodes + 31) / 32;
+    S.maxLevels = T.maxLevels; S.maxNodeLeaves = T.maxNodeLeaves; S.AS = T.AS; S.directLeaf = T.uniqueLeafIdx ? 1 : 0;
+#define X(name) dev.name = uploadStatic(T.name);
+    HIVED_STATIC_ARRAYS(X)
+#undef X
+#define Y(name, count, init)                                                                          \
+  {                                                                                                   \
+    size_t cnt_ = (size_t)(count);                                                                    \
+    dev.name = fill ? allocFill<int32_t>(cnt_, (int32_t)(init)) : allocOnly<int32_t>(cnt_);           \
+    mutableRegions.push_back({dev.name, (cnt_ ? cnt_ : 1) * sizeof(int32_t)});                        \
+  }
+    HIVED_MUTABLE_ARRAYS(Y)
+#undef Y
+    if (allocFailed) return outOfMemory();  // before anything is copied into a null array
+    dev.g_state.b = dev.g_vc.b = dev.g_prio.b = dev.g_flags.b = dev.g_nmem.b = dev.g_npre.b = dev.g_hdr;
+    dev.g_mem_leaf.b = dev.g_mem_pods.b = dev.g_hdr;
+    dev.stats = fill ? allocFill<long long>(ST_COUNT, 0) : allocOnly<long long>(ST_COUNT);
+    mutableRegions.push_back({dev.stats, ST_COUNT * sizeof(long long)});
+    dev.epoch = fill ? allocFill<int32_t>(MAX_CTAS, 1) : allocOnly<int32_t>(MAX_CTAS);
+    mutableRegions.push_back({dev.epoch, MAX_CTAS * sizeof(int32_t)});
+    dev.progress = allocFill<int32_t>(MAX_CTAS, 0);
+    if (allocFailed) return outOfMemory();
+    {
+      std::vector<Scratch> sc(nCtaMax);
+      for (int c = 0; c < nCtaMax; c++) {
+#define Z(name, count) sc[c].name = allocFill<int32_t>((size_t)(count), 0);
+        HIVED_SCRATCH_ARRAYS(Z)
+#undef Z
+      }
+      Scratch* dsc = (Scratch*)bk_alloc(sizeof(Scratch) * nCtaMax);
+      if (!dsc || allocFailed) { if (dsc) bk_free(dsc); return outOfMemory(); }
+      bk_h2d(dsc, sc.data(), sizeof(Scratch) * nCtaMax);
+      allocs.push_back(dsc);
+      dev.scratch = dsc;
+    }
     dScalars.ensure(MAX_CTAS * sizeof(CtaWords));
     dOwn.ensure(64);
     dPool.ensure(4096 * 4);
     dResults.ensure(sizeof(hived_result_t));
     dEvents.ensure(sizeof(hived_event_t));
-    poolOff = 0;
-    if (allocFailed || buffersFailed()) {
-      err = "out of device memory while creating the context (see hived_options_t: the group tables grow with "
-            "max_groups * max_group_leaves)";
-      return HIVED_ERR_CAPACITY;
+    if (allocFailed || buffersFailed()) return outOfMemory();
+    return 0;
+  }
+  template <typename TT>
+  TT* allocOnly(size_t count) {
+    TT* p = (TT*)bk_alloc((count ? count : 1) * sizeof(TT));
+    if (!p) { allocFailed = true; return nullptr; }
+    allocs.push_back(p);
+    return p;
+  }
+
+  // A context that answers every later call as `src` would (include/hived_clone.h).  `src`'s state in full: its device
+  // arrays through bk_copy_ctx, the host state below.  Every member of Engine is one of
+  //   copied:      T, opt (but device and flags), nCtaMax, the mutable device arrays (mutableRegions: the scheduler
+  //                state, dev.stats, dev.epoch), nodeBadHost, badCount, nBad, groupVcHost, groupStamp, batchStamp,
+  //                prioMaskHost, everRecovered, nPinnedOrder, hash, hashing (off with HIVED_OPT_NO_RESULT_HASH),
+  //                multiBatches;
+  //   per-context: dev (the clone's own pointers; dev.calm is set by every batch's prepare()), err, allocs,
+  //                mutableRegions' pointers, savedRegions and savedHash (no bench save slot), the staging buffers
+  //                (dEvents .. dOwn, dPool2, dScan) and what a staged batch leaves in them (poolOff, launchCta, ownHost,
+  //                ownOff, poolBase, poolEnd, ownerOf, canonicalDone, canonicalTotal, stagedEvents, stagedN,
+  //                poolCapWords, hasSugg, hasAux: rewritten by setStaged() before any batch reads them), the
+  //                multi-GPU partition's state (mg*: a staged source is refused), dev.progress (armProgress() writes
+  //                it before every run that reads it), the timing, launch and turn counters, stream, allocFailed and
+  //                deviceOrdinal.
+  // The device program keeps nothing else between batches: the per-CTA scratch (dev.scratch) is written by a decision
+  // before it reads it (vx_* are valid only where vx_stamp equals the CTA's epoch, both copied), and the bucket heads
+  // a CTA caches in shared memory (Sm::bkc_sched) are dropped at the start of every run and every resident kernel.
+  // A member added to Engine belongs in one of the two lists.
+  int cloneFrom(const Engine& src, int device, int flags) {
+    opt = src.opt;
+    opt.device = device < 0 ? src.deviceOrdinal : device;
+    opt.flags = flags;
+    deviceOrdinal = opt.device;
+    int rc = bk_init(deviceOrdinal, err);
+    if (rc) return rc;
+    T = src.T;
+    nCtaMax = src.nCtaMax;
+    rc = allocate(false);
+    if (rc) return rc;
+    std::vector<void*> dst(mutableRegions.size());
+    std::vector<const void*> from(mutableRegions.size());
+    std::vector<size_t> bytes(mutableRegions.size());
+    for (size_t i = 0; i < mutableRegions.size(); i++) {
+      dst[i] = mutableRegions[i].first;
+      from[i] = src.mutableRegions[i].first;
+      bytes[i] = mutableRegions[i].second;
     }
-    rc = launchProgram(*this, 0, true);
-    if (rc) { if (err.empty()) err = "device initialisation failed"; return rc; }
+    rc = bk_copy_ctx(*this, src, dst.data(), from.data(), bytes.data(), (int)dst.size());
+    if (rc) return rc;
+    nodeBadHost = src.nodeBadHost;
+    badCount = src.badCount;
+    nBad = src.nBad;
+    groupVcHost = src.groupVcHost;
+    groupStamp = src.groupStamp;
+    batchStamp = src.batchStamp;
+    prioMaskHost = src.prioMaskHost;
+    everRecovered = src.everRecovered;
+    nPinnedOrder = src.nPinnedOrder;
+    hash = src.hash;
+    hashing = src.hashing && !(flags & HIVED_OPT_NO_RESULT_HASH);
+    multiBatches = src.multiBatches;
     if (opt.flags & HIVED_OPT_CONCURRENT) return bk_open_concurrent(*this);
     return 0;
   }
@@ -703,6 +776,12 @@ int bk_launch_many(Engine* const* es, int k) {
   return 0;
 }
 #endif
+#ifndef HIVED_BK_COPY_CTX
+int bk_copy_ctx(Engine&, const Engine&, void* const* to, const void* const* from, const size_t* bytes, int n) {
+  for (int i = 0; i < n; i++) bk_d2d(to[i], from[i], bytes[i]);
+  return 0;
+}
+#endif
 #ifndef HIVED_BK_CONCURRENT
 int bk_open_concurrent(Engine&) { return 0; }
 bool bk_batch_begin(Engine&) { return false; }
@@ -728,6 +807,19 @@ int hived_create(const char* spec_text, const hived_options_t* opt, hived_ctx** 
   *out = nullptr;
   auto ctx = std::make_unique<hived_ctx>();
   int rc = ctx->e.create(spec_text, opt);
+  if (rc) { g_hived_create_error = ctx->e.err; return rc; }
+  *out = ctx.release();
+  return 0;
+}
+// ---- include/hived_clone.h
+int hived_clone(hived_ctx* src, int32_t device, int32_t flags, hived_ctx** out) {
+  *out = nullptr;
+  if (!src->e.mgCursor.empty()) {
+    g_hived_create_error = "hived_clone: the source is staged for a multi-GPU partition";
+    return HIVED_ERR_BAD_SPEC;
+  }
+  auto ctx = std::make_unique<hived_ctx>();
+  int rc = ctx->e.cloneFrom(src->e, device, flags);
   if (rc) { g_hived_create_error = ctx->e.err; return rc; }
   *out = ctx.release();
   return 0;

@@ -594,6 +594,18 @@ class BatchContext:
             raise RuntimeError("hived_create failed (%d): %s" % (rc, (lib.hived_create_error() or b"").decode()))
         self.n_nodes = lib.hived_num_nodes(self.ctx)
 
+    def clone(self, device: int = -1, flags: int = 0) -> "BatchContext":
+        """hived_clone (include/hived_clone.h): a new BatchContext over an independent copy of this one's context."""
+        out = C.c_void_p()
+        rc = _cabi.bind_clone(self.lib).hived_clone(self.ctx, device, flags, C.byref(out))
+        if rc != 0:
+            raise RuntimeError("hived_clone failed (%d): %s" % (rc, (self.lib.hived_create_error() or b"").decode()))
+        bc = BatchContext.__new__(BatchContext)
+        bc.lib, bc.ctx, bc.n_nodes = self.lib, out, self.n_nodes
+        bc.opt = _cabi.Options.from_buffer_copy(self.opt)
+        bc.opt.device, bc.opt.flags = self.opt.device if device < 0 else device, flags
+        return bc
+
     def set_all_nodes_healthy(self):
         """Healthy nodes arrive in ascending node id (= name) order (SURVEY.md Appendix A item 10)."""
         ev = np.zeros(self.n_nodes, dtype=EVENT_DT)
